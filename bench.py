@@ -20,11 +20,16 @@ and the process exits non-zero on a mismatch.
 
   --impl reference   times the CPU oracle instead (the reference is Go; no Go toolchain exists here or on the
                      GPU box, so the "reference arm" is the restatement in oracle/, all host threads).
+
+  --dump-outputs DIR writes what each action of the last timed step returned to its caller (kai_result) as
+                     DIR/<action>.<field>.npy, float64; the synthetic inputs are seeded, so two builds run with the same
+                     arguments can be compared array by array.
 """
 from __future__ import annotations
 
 import argparse
 import ctypes as C
+import dataclasses
 import json
 import os
 import subprocess
@@ -43,6 +48,7 @@ from kai_scheduler_b200 import abi, synthetic  # noqa: E402
 METRIC = "pods_placed_per_sec"
 UNIT = "pods/s"
 BYTES_PER_NODE = (2 * 4 + 1) * 8 + 4  # SURVEY.md §8d: Idle[R]+Releasing[R]+Allocatable[1] f64 + 4 B flags, R=4
+DUMP_LIMIT_BYTES = 64 << 20  # --dump-outputs: larger outputs are written as a fixed, seeded sample
 
 
 def measured_peak_gbs():
@@ -52,7 +58,25 @@ def measured_peak_gbs():
             return float(json.load(open(p))["hbm_gbs"]), "measured"
         except Exception:
             pass
-    return 6650.0, "fallback"
+    return 3350.0, "H100 SXM data sheet"
+
+
+def dump_outputs(directory, results):
+    """results: {action: abi.Result}.  One float64 .npy per array (ints are exact in f64); when the whole set is over
+    DUMP_LIMIT_BYTES every array is cut to the same fraction of its flattened elements, chosen with a fixed seed."""
+    arrays = {}
+    for action, res in results.items():
+        for f in dataclasses.fields(res):
+            arrays[f"{action}.{f.name}"] = np.asarray(getattr(res, f.name), dtype=np.float64)
+    total = sum(a.nbytes for a in arrays.values())
+    frac = min(1.0, DUMP_LIMIT_BYTES / total) if total else 1.0
+    os.makedirs(directory, exist_ok=True)
+    for name, a in arrays.items():
+        if frac < 1.0:
+            flat = a.reshape(-1)
+            keep = np.sort(np.random.default_rng(0).choice(flat.size, size=int(flat.size * frac), replace=False))
+            a = flat[keep]
+        np.save(os.path.join(directory, f"{name}.npy"), a)
 
 
 class ClockSampler(threading.Thread):
@@ -170,7 +194,11 @@ def main():
     ap.add_argument("--snapshot", default=None,
                     help="time a recorded cluster instead of a synthetic config: a zip of the reference's snapshot "
                          "plugin (kai_scheduler_b200/snapshot_io.py); actions and plugin arguments come from the file")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write each action's result of the last timed step to DIR/<action>.<field>.npy (float64)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     args.warmup = max(args.warmup, 0)
     rank, world, local = dist_env()
 
@@ -245,9 +273,11 @@ def main():
             dist.barrier()
         torch.cuda.synchronize()
 
-    def one_step():
-        """returns (device_ms, e2e_s, pods, stats)"""
+    def one_step(keep=None):
+        """returns (device_ms, e2e_s, pods, stats); keep: dict that receives a copy of every action's result, copied
+        outside the e2e time"""
         t0 = time.perf_counter()
+        t_keep = 0.0
         eng.load_c(c_snap, snap.n_res)       # H2D of the whole snapshot + open-session kernels
         dev, moved, launches_, alg_, act_ = 0.0, 0, 0, 0, 0.0
         one_step.evicted, one_step.decisions = 0, 0
@@ -261,7 +291,11 @@ def main():
             launches_ = int(st.kernel_launches)
             alg_ += int(st.algorithmic_bytes)
             act_ += st.action_ms
-        e2e = time.perf_counter() - t0
+            if keep is not None:  # the next action overwrites the engine-owned arrays r points into
+                tk = time.perf_counter()
+                keep[a] = abi.Result.from_c(r, snap.n_res)
+                t_keep += time.perf_counter() - tk
+        e2e = time.perf_counter() - t0 - t_keep
         st.kernel_launches, st.algorithmic_bytes, st.action_ms = launches_, alg_, act_
         return st.open_session_ms + dev, e2e, moved, st, r
 
@@ -274,8 +308,9 @@ def main():
     phase_ms = {"upload": 0.0, "open_session": 0.0, "action": 0.0, "download": 0.0}
     t_wall0 = time.perf_counter()
     decisions = evicted_e = 0
-    for _ in range(args.steps):
-        d, e, p, st, r = one_step()
+    kept = {}
+    for i in range(args.steps):
+        d, e, p, st, r = one_step(kept if args.dump_outputs and i == args.steps - 1 else None)
         decisions, evicted_e = one_step.decisions, one_step.evicted
         dev_ms += d
         e2e_s += e
@@ -292,6 +327,8 @@ def main():
     wall = time.perf_counter() - t_wall0
     clocks = sampler.stop()
     last = abi.Result.from_c(r, snap.n_res)  # outcome of the last timed step (copied out of the engine's buffers)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, kept)
     ranks_agree = True
     if world > 1:  # every rank runs the same sequencer over its node stripe: the bindings must be identical everywhere
         import hashlib
@@ -317,14 +354,7 @@ def main():
         peak, which = measured_peak_gbs()
         sweep_bytes = sweep_rows * BYTES_PER_NODE
         achieved = sweep_bytes / (sweep_ms * 1e-3) / 1e9 if sweep_ms > 0 else 0.0
-        traffic, traffic_src = None, "no ncu --set full capture recorded for this build"
-        tp = os.path.join(ROOT, "profiles", "r02_k_record_traffic.json")
-        if os.path.exists(tp):
-            try:
-                tj = json.load(open(tp))
-                traffic, traffic_src = tj["dram_bytes_per_launch"], tj["source"]
-            except Exception:
-                pass
+        traffic, traffic_src = None, "not measured (no DRAM counter capture recorded for this build)"
         line = {
             "metric": METRIC, "value": pods_all / (dev_ms * 1e-3), "unit": UNIT, "n_gpus": args.gpus,
             "steps": args.steps, "warmup": max(args.warmup, 3), "ms_per_step": dev_ms / args.steps,
@@ -339,7 +369,7 @@ def main():
                     "phases_ms": {k: v / max(args.steps, 1) for k, v in phase_ms.items()}},
             "gpu_launches": launches,
             "roofline": {"bound": "hbm", "kernel": "k_record (one node-table sweep per launch: node deltas, fit + score of every row, "
-                                                   "per-scanner top-M; 74 % of the GPU time of a step, profiles/r02_launches_bench.csv)",
+                                                   "per-scanner top-M; its share of the action time is sweep_share_of_step)",
                          "achieved": achieved, "peak": peak, "unit": "GB/s",
                          "frac": achieved / peak, "peak_source": which + " (MEASURED_PEAKS.json hbm_gbs)",
                          "algorithmic_bytes_per_launch": sweep_bytes, "rows_per_launch": sweep_rows,

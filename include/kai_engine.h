@@ -1,5 +1,5 @@
 /*
- * kai_engine.h — C ABI of libkaigpu.so, the B200-native scheduling-cycle engine.
+ * kai_engine.h — C ABI of libkaigpu.so, the H100-native scheduling-cycle engine.
  *
  * This is the drop-in boundary for ONE hot path of NVIDIA/KAI-Scheduler: the
  * per-Session scheduling cycle in pkg/scheduler.  A Go `framework.Action`

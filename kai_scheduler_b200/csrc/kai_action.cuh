@@ -2046,8 +2046,8 @@ __global__ void __launch_bounds__(kMergeThreads, 1) k_merge(const __grid_constan
   }
 }
 
-// The same merge on a thread-block cluster (Blackwell: 4 CTAs x 256 threads on 4 SMs, one candidate per thread): the
-// 55-step network is bound by instruction issue, so four SMs run it ~3x faster than one.  Partner exchange: warp shuffle
+// The same merge on a thread-block cluster (Hopper: 4 CTAs x 256 threads on 4 SMs, one candidate per thread): the
+// 55-step network is bound by instruction issue, so four SMs share it instead of one.  Partner exchange: warp shuffle
 // below 32 lanes, the CTA's shared memory below 256, the partner CTA's shared memory (distributed shared memory,
 // cluster.map_shared_rank) for the three steps with j >= 256; every CTA streams its own quarter of the sorted prefix to
 // host memory, CTA 0 writes the header after the cluster barrier.

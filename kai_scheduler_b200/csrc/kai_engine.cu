@@ -293,7 +293,7 @@ int kai_engine_create(const kai_config *cfg, kai_engine **out) {
     delete e;
     return KAI_ERR_NO_DEVICE;
   }
-  if (prop.major < 10) {  // sm_100a cubin only
+  if (prop.major != 9 || prop.minor != 0) {  // sm_90a cubin only: it loads on compute capability 9.0 and nothing else
     delete e;
     return KAI_ERR_NO_DEVICE;
   }
@@ -816,7 +816,7 @@ int kai_engine_load_snapshot(kai_engine *e, const kai_snapshot *s) {
   e->visits_cap = std::max(16, 2 * J + T + 16);
   {  // launch transport: scanners = CTAs of k_record; k_merge sorts scanners x kTopM candidates (<= kMergeThreads)
     int lg = 1;
-    while (lg * 2 <= std::min(2 * e->num_sms, kMergeThreads / kTopM)) lg *= 2;  // 256 on B200: a power of two keeps the merge sort full
+    while (lg * 2 <= std::min(2 * e->num_sms, kMergeThreads / kTopM)) lg *= 2;  // 256 on H100 (132 SMs): a power of two keeps the merge sort full
     if (const char *g = getenv("KAI_LAUNCH_GRID")) {
       int v = atoi(g);
       if (v >= 1) lg = std::min(v, kMergeThreads / kTopM);

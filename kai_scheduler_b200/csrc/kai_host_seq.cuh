@@ -9,10 +9,10 @@
 //     mapped memory to the scanners' device-side record buffer, the scanners keep their node tiles in shared memory and
 //     answer every record with tagged 128-bit words written straight into pinned host memory.
 //
-// Why: measured on B200 (profiles/microbench, profiles/r01_sequencer_modes.md) one GPU lane needs ~20k
-// cycles (10 us) of dependent L1/L2/shared-memory latencies per job for the pointer-chasing part of the
-// cycle (heap pops, DRF keys, statement log); a host core does the same in a few hundred ns.  The O(N)
-// work per allocateTask — the node sweep — stays on the GPU in both modes.
+// Why: the pointer-chasing part of the cycle (heap pops, DRF keys, statement log) is a chain of dependent
+// L1/L2/shared-memory accesses per job (latencies in profiles/microbench) on a single GPU lane; a host core
+// serves the same chain from its caches far faster.  The O(N) work per allocateTask — the node sweep — stays
+// on the GPU in both modes.
 #pragma once
 #include <algorithm>
 #include <chrono>

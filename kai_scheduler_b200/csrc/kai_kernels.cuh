@@ -1,4 +1,4 @@
-// kai_kernels.cuh — sm_100a kernels of the scheduling-cycle engine.
+// kai_kernels.cuh — sm_90a kernels of the scheduling-cycle engine.
 //
 //   k_node_totals    Σ node Allocatable over ready nodes          (proportion.go:252-288)
 //   k_queue_usage    per-queue Allocated / Request scatter-add    (proportion.go:347-401)

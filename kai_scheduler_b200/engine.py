@@ -24,7 +24,7 @@ def lib() -> C.CDLL:
         if not os.path.exists(LIB_PATH):
             raise FileNotFoundError(
                 f"{LIB_PATH} is missing: run `python -c 'import __graft_entry__ as g; g.build()'` "
-                "(nvcc, sm_100a).  There is no CPU fallback.")
+                "(nvcc, sm_90a).  There is no CPU fallback.")
         _LIB = C.CDLL(LIB_PATH)
         abi.bind_engine_api(_LIB, "kai_engine")
         _LIB.kai_last_error.argtypes = [C.c_void_p]

@@ -1,10 +1,10 @@
 #!/usr/bin/env python
-"""Transcribe the reference's Go table tests into JSON fixtures (run in the build container only).
+"""Transcribe the reference's Go table tests into JSON fixtures.
 
-    python tests/golden/gen_fixtures.py            # rewrites tests/golden/*.json
+    KAI_REFERENCE=<KAI-Scheduler checkout> python tests/golden/gen_fixtures.py   # rewrites tests/golden/*.json
 
-Reads /root/reference (read-only) and writes small JSON files next to this script.
-The fixtures, not the reference, travel to the GPU box.  Sources transcribed:
+Reads the reference checkout (read-only) and writes small JSON files next to this script.
+The tests read the fixtures only, never the reference.  Sources transcribed:
 
   actions/*.json          pkg/scheduler/actions/{allocate,reclaim,consolidation}/*_test.go and
                           pkg/scheduler/actions/integration_tests/{allocate,reclaim,consolidation,
@@ -30,7 +30,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
 from go_literal import find_literals  # noqa: E402
 
-REF = "/root/reference/pkg/scheduler"
+REF = os.path.join(os.environ.get("KAI_REFERENCE", "."), "pkg", "scheduler")
 
 IDENTS = {
     "constants.PriorityTrainNumber": 50,

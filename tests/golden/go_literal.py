@@ -1,8 +1,8 @@
 """Minimal parser for Go composite literals, enough for the reference's table tests.
 
-Used ONLY by tests/golden/gen_fixtures.py, which runs in the build container
-where /root/reference is mounted, to transcribe the reference's Go test tables
-into JSON fixtures.  Nothing at test run time imports this.
+Used ONLY by tests/golden/gen_fixtures.py, which reads a checkout of the
+reference to transcribe its Go test tables into JSON fixtures.  Nothing at
+test run time imports this.
 
 Grammar handled:
     value   := string | rawstring | number | '-' number | ident ('.' ident)* [call | literal]

@@ -16,7 +16,7 @@ def test_record_packing_and_multi_gpu_list_merge():
     src = os.path.join(ROOT, "tests", "native", "launch_host_check.cu")
     with tempfile.TemporaryDirectory() as d:
         exe = os.path.join(d, "check")
-        subprocess.check_call(["nvcc", "-O1", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-x", "cu", "-o", exe, src],
+        subprocess.check_call(["nvcc", "-O1", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-x", "cu", "-o", exe, src],
                               stdout=subprocess.DEVNULL)
         out = subprocess.run([exe], capture_output=True, text=True)
     assert out.returncode == 0, out.stdout + out.stderr

@@ -109,7 +109,7 @@ VICTIM_WORKLOADS = [
 @pytest.mark.parametrize("kw", VICTIM_WORKLOADS, ids=[f"n{k['n_nodes']}q{k['victim_queues']}j{k['reclaimer_jobs']}" for k in VICTIM_WORKLOADS])
 def test_moved_victims_keep_one_entry_per_node(kw):
     """Victim workloads where consolidation moves a victim (A -> B) and a later statement evicts it on B and re-places it
-    on C: the task holds entries on three nodes (found on B200: oracle and engine both kept only two and disagreed).  The
+    on C: the task holds entries on three nodes (found on the GPU: oracle and engine both kept only two and disagreed).  The
     result carries one (node, status) per task, so the clones the nodes hold are read from the oracle (test-only export)
     and checked both ways: the node vectors follow from the entries, and every placed task of the result has its entry."""
     snap = synthetic.reclaim_snapshot(**kw)

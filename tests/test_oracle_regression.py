@@ -1,7 +1,7 @@
 """Digest regression of the oracle on the synthetic workloads the GPU parity tests use (CPU).
 
 The engine is compared with the oracle on these snapshots on the GPU box; here the oracle's own outcome is pinned by a
-digest recorded when engine and oracle last agreed on B200 (tests/golden/oracle_digests.json), so that a change to the
+digest recorded when engine and oracle last agreed on the GPU (tests/golden/oracle_digests.json), so that a change to the
 oracle that would silently move it away from the engine is caught without a GPU.  Regenerate with
 `python tests/test_oracle_regression.py --record` only together with a green `pytest -m gpu` run.
 """

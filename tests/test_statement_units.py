@@ -155,7 +155,7 @@ def test_statement_checkpoint_rollback(name, ops):
 def test_one_clone_per_node_is_unbounded():
     """NodeInfo.PodInfos is a map per node (node_info.go:400-402): a pod that is evicted on A, pipelined to B, evicted
     there and pipelined to C holds a clone on each of the three nodes (Releasing, Releasing, Pipelined); Discard walks
-    back through all of them.  (Round 2: oracle and engine used to keep two entries and disagreed on B200.)"""
+    back through all of them.  (Round 2: oracle and engine used to keep two entries and disagreed.)"""
     topo = {"Nodes": {f"node{i}": {"GPUs": 2} for i in range(3)}, "Queues": [{"Name": "queue0", "DeservedGPUs": 6}],
             "Jobs": [job("running_job0", "Running", "node0")]}
     snap, _ = dsl.build_snapshot(topo)

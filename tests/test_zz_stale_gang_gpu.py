@@ -1,4 +1,4 @@
-"""stalegangeviction with a grace period on the engine (B200): the reference's own table
+"""stalegangeviction with a grace period on the engine (GPU): the reference's own table
 (actions/stalegangeviction/stalegangeviction_test.go, grace period 60 s, per-job staleness timestamps) through the C ABI,
 against the oracle and against the table's expectations; plus the grace-period variations on a synthetic cluster.
 
