@@ -55,6 +55,14 @@ struct __align__(64) JobRec {
   int pad[3];
 };
 
+// Order-independence test of the open-session sums (k_node_totals / k_queue_usage), zeroed by every load.
+// Index 0 = node totals, 1 = queue usage.
+struct OpenSums {
+  unsigned long long sum_abs[2][3];  // per resource: sum of |summand| over the integer-valued summands (saturating)
+  unsigned int inexact[2];           // bit r: resource r has a summand that is not an integer of at most 2^53
+  unsigned int blocks_done[2];       // last-block ticket
+};
+
 // Immutable (per cycle) device snapshot + session state pointers.  Passed by value to kernels.
 struct DevSnap {
   int R, N, Q, J, S, T, NPC, mask_words;
@@ -76,6 +84,7 @@ struct DevSnap {
   const int *q_child_begin, *q_children;                 // CSR of children (ascending index)
   const int *top_queues;                                 // [n_top]
   const int *level_group_begin, *level_groups;           // fair-share: groups (parent queue or -1) per level
+  const int *q_task_begin, *q_tasks;                     // CSR: device indices of the tasks under each queue, caller order
   const int *q_job_begin;                                // [Q+1] leaf-heap arena offsets
   const int *q_jobs_sorted;                              // [J] jobs grouped by queue, (priority desc, order_rank)
   // jobs
@@ -90,6 +99,7 @@ struct DevSnap {
   unsigned char *t_virtual;                // session state
   const uint32_t *pred_mask;
   double *total;  // [3] device
+  OpenSums *osum;
   // ---- written by the fair-share / prepare kernels (device only) ----
   double *q_allocatable;  // [3][Q] GetAllocatableShare per queue (static within a cycle)
   unsigned long long *j_key0;  // [J] JobOrderFn sort key at action start

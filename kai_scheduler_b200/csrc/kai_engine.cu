@@ -312,6 +312,7 @@ static int load_tail(kai_engine *e, const kai_snapshot *s, int n_dom_levels, boo
   if (T > 0) {
     int blocks = std::min(e->num_sms * 8, (T + 255) / 256);
     k_queue_usage<<<blocks, 256, 0, e->stream>>>(ds);
+    if (Q > 0) k_queue_usage_ordered<<<(QR * Q + 7) / 8, 256, 0, e->stream>>>(ds);  // exits at once when exact
   }
   if (Q > 0) k_fair_share<<<1, 1024, 0, e->stream>>>(ds, e->cfg.k_value, e->fs_w, e->fs_rr);
   cudaEventRecord(e->ev[2], e->stream);
@@ -322,7 +323,7 @@ static int load_tail(kai_engine *e, const kai_snapshot *s, int n_dom_levels, boo
   e->stats.upload_ms = ms;
   cudaEventElapsedTime(&ms, e->ev[1], e->ev[2]);
   e->stats.open_session_ms = ms;
-  e->stats.kernel_launches = (N > 0) + (T > 0) + (Q > 0);
+  e->stats.kernel_launches = (N > 0) + (T > 0) + (T > 0 && Q > 0) + (Q > 0);
   e->stats.action_ms = 0;
   e->stats.download_ms = 0;
   e->stats.decisions = e->stats.nodes_scanned = e->stats.algorithmic_bytes = 0;
@@ -701,6 +702,21 @@ int kai_engine_load_snapshot(kai_engine *e, const kai_snapshot *s) {
   size_t o_psjob = reserve_up((size_t)std::max(S, 1) * 4);
   size_t o_treq = reserve_up((size_t)std::max(T, 1) * R * 8);
   size_t o_tjob = reserve_up((size_t)std::max(T, 1) * 4), o_tps = reserve_up((size_t)std::max(T, 1) * 4);
+  // tasks under each queue (itself and every ancestor of the job's queue) in the caller's task order, as device indices:
+  // the order k_queue_usage_ordered adds them in (the oracle goes by job, podset, task)
+  std::vector<int> q_task_begin(Q + 1, 0), q_tasks;
+  {
+    std::vector<int> dev_of(std::max(T, 1));
+    for (int i = 0; i < T; i++) dev_of[perm[i]] = i;
+    for (int t = 0; t < T; t++)
+      for (int a = s->job_queue[t_job[t]]; a >= 0; a = s->queue_parent[a]) q_task_begin[a + 1]++;
+    for (int q = 0; q < Q; q++) q_task_begin[q + 1] += q_task_begin[q];
+    q_tasks.assign(std::max(q_task_begin[Q], 1), 0);
+    std::vector<int> fill(q_task_begin.begin(), q_task_begin.end() - 1);
+    for (int t = 0; t < T; t++)
+      for (int a = s->job_queue[t_job[t]]; a >= 0; a = s->queue_parent[a]) q_tasks[fill[a]++] = dev_of[t];
+  }
+  size_t o_qtb = reserve_up((size_t)(Q + 1) * 4), o_qtasks = reserve_up(q_tasks.size() * 4);
   size_t o_tnom = s->task_nominated ? reserve_up((size_t)std::max(T, 1) * 4) : 0;
   size_t o_tpc = s->task_pred_class ? reserve_up((size_t)std::max(T, 1) * 4) : 0;
   size_t o_tst = reserve_up((size_t)std::max(T, 1) * 4), o_tnode = reserve_up((size_t)std::max(T, 1) * 4);
@@ -719,7 +735,7 @@ int kai_engine_load_snapshot(kai_engine *e, const kai_snapshot *s) {
   // device-only region
   size_t o_tvirt = reserve_up((size_t)std::max(T, 1));
   size_t o_qfair = reserve_up(QN * 8), o_qreq = reserve_up(QN * 8), o_qal = reserve_up(QN * 8), o_qalnp = reserve_up(QN * 8);
-  size_t o_total = reserve_up(3 * 8);
+  size_t o_total = reserve_up(3 * 8), o_osum = reserve_up(sizeof(OpenSums));
   size_t o_qla = reserve_up(QN * 8);
   size_t o_jkey = reserve_up((size_t)std::max(J, 1) * 8), o_leafs = reserve_up((size_t)std::max(J, 1) * 4);
   size_t o_leafc = reserve_up((size_t)std::max(Q, 1) * 4), o_pscnt = reserve_up((size_t)3 * std::max(S, 1) * 4);
@@ -787,6 +803,8 @@ int kai_engine_load_snapshot(kai_engine *e, const kai_snapshot *s) {
   }
   put(o_tjob, t_job.data(), (size_t)T * 4);
   put(o_tps, t_podset.data(), (size_t)T * 4);
+  put(o_qtb, q_task_begin.data(), (size_t)(Q + 1) * 4);
+  put(o_qtasks, q_tasks.data(), q_tasks.size() * 4);
   if (s->task_nominated) {
     int *x = (int *)(h + o_tnom);
     for (int t = 0; t < T; t++) x[t] = s->task_nominated[perm[t]];
@@ -849,6 +867,8 @@ int kai_engine_load_snapshot(kai_engine *e, const kai_snapshot *s) {
   ds.top_queues = (const int *)(d + o_top);
   ds.level_group_begin = (const int *)(d + o_lgb);
   ds.level_groups = (const int *)(d + o_lg);
+  ds.q_task_begin = (const int *)(d + o_qtb);
+  ds.q_tasks = (const int *)(d + o_qtasks);
   ds.q_job_begin = (const int *)(d + o_qjb);
   ds.q_jobs_sorted = (const int *)(d + o_qjs);
   ds.j_queue = (const int *)(d + o_jq);
@@ -870,6 +890,7 @@ int kai_engine_load_snapshot(kai_engine *e, const kai_snapshot *s) {
   ds.t_virtual = (unsigned char *)(d + o_tvirt);
   ds.pred_mask = (s->pred_mask && NPC > 0) ? (const uint32_t *)(d + o_mask) : nullptr;
   ds.total = (double *)(d + o_total);
+  ds.osum = (OpenSums *)(d + o_osum);
   ds.q_allocatable = (double *)(d + o_qla);
   ds.j_key0 = (unsigned long long *)(d + o_jkey);
   ds.leaf_sorted = (int *)(d + o_leafs);
@@ -897,9 +918,9 @@ int kai_engine_load_snapshot(kai_engine *e, const kai_snapshot *s) {
     rb(h_.foreign); rb(h_.q_parent); rb(h_.q_priority); rb(h_.q_uid_rank); rb(h_.q_nchildren); rb(h_.q_creation);
     rb(h_.q_deserved); rb(h_.q_limit); rb(h_.q_oqw); rb(h_.q_usage); rb(h_.q_fair); rb(h_.q_request); rb(h_.q_alloc);
     rb(h_.q_alloc_np); rb(h_.q_child_begin); rb(h_.q_children); rb(h_.top_queues); rb(h_.level_group_begin);
-    rb(h_.level_groups); rb(h_.q_job_begin); rb(h_.q_jobs_sorted); rb(h_.j_queue); rb(h_.j_priority);
+    rb(h_.level_groups); rb(h_.q_task_begin); rb(h_.q_tasks); rb(h_.q_job_begin); rb(h_.q_jobs_sorted); rb(h_.j_queue); rb(h_.j_priority);
     rb(h_.j_order_rank); rb(h_.j_ps_begin); rb(h_.j_flags); rb(h_.ps_min); rb(h_.ps_task_begin); rb(h_.ps_job);
-    rb(h_.t_req); rb(h_.t_job); rb(h_.t_podset); rb(h_.t_nominated); rb(h_.t_pred_class); rb(h_.t_status);
+    rb(h_.t_req); rb(h_.t_job); rb(h_.t_podset); rb(h_.osum); rb(h_.t_nominated); rb(h_.t_pred_class); rb(h_.t_status);
     rb(h_.t_node); rb(h_.t_node_status); rb(h_.t_virtual); rb(h_.pred_mask); rb(h_.total); rb(h_.q_allocatable);
     rb(h_.j_key0); rb(h_.leaf_sorted); rb(h_.leaf_count); rb(h_.ps_cnt0); rb(h_.j_req); rb(h_.j_req_valid);
     rb(h_.ops); rb(h_.tta); rb(h_.ps_order); rb(h_.hot_global); rb(h_.jrec);

@@ -1,7 +1,8 @@
 // kai_kernels.cuh — sm_90a kernels of the scheduling-cycle engine.
 //
-//   k_node_totals    Σ node Allocatable over ready nodes          (proportion.go:252-288)
-//   k_queue_usage    per-queue Allocated / Request scatter-add    (proportion.go:347-401)
+//   k_node_totals    Σ node Allocatable over ready nodes          (proportion.go:252-288)  } exact or in the
+//   k_queue_usage    per-queue Allocated / Request scatter-add    (proportion.go:347-401)  } oracle's order
+//   k_queue_usage_ordered  the oracle's order where k_queue_usage's sums could round      } (DESIGN.md §2)
 //   k_fair_share     hierarchical fair-share division per level   (resource_division.go:26-357)
 //   k_action         persistent cooperative kernel running a whole Action (allocate) on device:
 //                    node tiles resident in shared memory, one fit+score+argmax sweep per
@@ -46,16 +47,96 @@ __device__ __forceinline__ void ld_relaxed_b128(const void *p, unsigned long lon
 }
 
 // ---------------------------------------------------------------------------------------------
+// Exact-or-ordered rule of the open-session sums (DESIGN.md §2).  The oracle adds in ascending index order.  When every
+// summand of a resource is an integer and the sum of their magnitudes is at most 2^53, every partial sum of any subset,
+// in any order and association, is an exact integer, so the parallel tree + atomics below give the oracle's bits.
+// Otherwise that resource is redone in the oracle's order.
+// ---------------------------------------------------------------------------------------------
+constexpr unsigned long long kExactSat = (1ull << 53) + 1;  // sums of magnitudes saturate here: "above 2^53"
+__device__ __forceinline__ void note_summand(double v, int r, unsigned long long &sum, unsigned &inexact) {
+  const double a = fabs(v);
+  if (v == trunc(v) && a <= 9007199254740992.0)
+    sum = min(sum + (unsigned long long)a, kExactSat);
+  else
+    inexact |= 1u << r;  // fractional, above 2^53, inf or NaN
+}
+__device__ __forceinline__ bool sums_exact(const volatile OpenSums *os, int which, int r) {
+  return !((os->inexact[which] >> r) & 1u) && os->sum_abs[which][r] < kExactSat;
+}
+// Adds this block's flags and magnitude sums to os.  A block adds at most 256 * kExactSat < 2^62 and at most kExactSat
+// per block reaches the global counter, so it cannot wrap below 2048 blocks (the grids are at most 8 per SM).  With
+// want_last, returns true in the block that finished last, which then sees every block's sums and flags.
+__device__ bool open_sums_publish(OpenSums *os, int which, const unsigned long long *sum, unsigned inexact,
+                                  bool want_last) {
+  __shared__ unsigned long long ssum[QR];
+  __shared__ unsigned sbits;
+  __shared__ bool last;
+  if (threadIdx.x < QR) ssum[threadIdx.x] = 0;
+  if (threadIdx.x == 0) sbits = 0;
+  __syncthreads();
+  // a warp's 32 sums (each at most kExactSat) first, so that the shared atomics see one add per warp
+  for (int r = 0; r < QR; r++) {
+    unsigned long long x = sum[r];
+    for (int o = 16; o > 0; o >>= 1) x += __shfl_down_sync(0xffffffffu, x, o);
+    if ((threadIdx.x & 31) == 0 && x) atomicAdd(&ssum[r], x);
+  }
+  inexact = __reduce_or_sync(0xffffffffu, inexact);
+  if ((threadIdx.x & 31) == 0 && inexact) atomicOr(&sbits, inexact);
+  __syncthreads();
+  if (threadIdx.x < QR && ssum[threadIdx.x]) atomicAdd(&os->sum_abs[which][threadIdx.x], min(ssum[threadIdx.x], kExactSat));
+  if (threadIdx.x == 0 && sbits) atomicOr(&os->inexact[which], sbits);
+  if (!want_last) return false;
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0) last = atomicAdd(&os->blocks_done[which], 1u) == gridDim.x - 1;
+  __syncthreads();
+  if (last) __threadfence();
+  return last;
+}
+
+// One warp adds n summands in index order, NV sums side by side; lane 0 writes them to out.  The lanes stage a chunk of
+// summands in shared memory (their loads are independent and overlap), then lane 0 runs the add chain over the chunk.
+// get(k, v) fills v[] with the k-th summands; a summand that does not count stays +0.0, which leaves the sum unchanged:
+// a sum started at +0.0 is never -0.0 under round-to-nearest, and x + 0.0 == x for every other x.
+constexpr int kOrdChunk = 128;
+template <int NV, class F>
+__device__ void warp_ordered_sums(int n, F get, double (*buf)[kOrdChunk], double *out) {
+  const int lane = threadIdx.x & 31;
+  double acc[NV];
+  for (int c = 0; c < NV; c++) acc[c] = 0.0;
+  for (int base = 0; base < n; base += kOrdChunk) {
+    for (int i = lane; i < kOrdChunk; i += 32) {
+      double v[NV];
+      for (int c = 0; c < NV; c++) v[c] = 0.0;
+      if (base + i < n) get(base + i, v);
+      for (int c = 0; c < NV; c++) buf[c][i] = v[c];
+    }
+    __syncwarp();
+    if (lane == 0) {
+      const int m = min(kOrdChunk, n - base);
+      for (int i = 0; i < m; i++)
+        for (int c = 0; c < NV; c++) acc[c] = __dadd_rn(acc[c], buf[c][i]);
+    }
+    __syncwarp();
+  }
+  if (lane == 0)
+    for (int c = 0; c < NV; c++) out[c] = acc[c];
+}
+
+// ---------------------------------------------------------------------------------------------
 // K_totals: proportion.setTotalResources (proportion.go:252-288)
 // ---------------------------------------------------------------------------------------------
 __global__ void k_node_totals(DevSnap s) {
   double acc[QR] = {0, 0, 0};
+  unsigned long long mag[QR] = {0, 0, 0};
+  unsigned inexact = 0;
   for (int n = blockIdx.x * blockDim.x + threadIdx.x; n < s.N; n += gridDim.x * blockDim.x) {
     if (!(s.nflags[n] & KAI_NODE_READY)) continue;
     for (int r = 0; r < QR; r++) {
       double v = s.alloc[(size_t)r * s.N + n];
       if (s.foreign) v = __dsub_rn(v, s.foreign[(size_t)r * s.N + n]);
       acc[r] = __dadd_rn(acc[r], v);
+      note_summand(v, r, mag[r], inexact);
     }
   }
   __shared__ double sh[QR][32];
@@ -70,18 +151,35 @@ __global__ void k_node_totals(DevSnap s) {
     for (int w = 0; w < (blockDim.x + 31) / 32; w++) v = __dadd_rn(v, sh[threadIdx.x][w]);
     atomicAdd(&s.total[threadIdx.x], v);
   }
+  if (!open_sums_publish(s.osum, 0, mag, inexact, true)) return;
+  // last block: warp r redoes resource r in ascending node index, as the oracle adds
+  __shared__ double buf[QR][1][kOrdChunk];
+  const int r = threadIdx.x >> 5;
+  if (r >= QR || sums_exact(s.osum, 0, r)) return;
+  double out;
+  warp_ordered_sums<1>(s.N, [&](int n, double *v) {
+    if (!(s.nflags[n] & KAI_NODE_READY)) return;
+    double x = s.alloc[(size_t)r * s.N + n];
+    if (s.foreign) x = __dsub_rn(x, s.foreign[(size_t)r * s.N + n]);
+    v[0] = x;
+  }, buf[r], &out);
+  if ((threadIdx.x & 31) == 0) s.total[r] = out;
 }
 
 // ---------------------------------------------------------------------------------------------
 // K_usage: proportion.updateQueuesCurrentResourceUsage (proportion.go:347-401)
 // ---------------------------------------------------------------------------------------------
 __global__ void k_queue_usage(DevSnap s) {
+  unsigned long long mag[QR] = {0, 0, 0};
+  unsigned inexact = 0;
   for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < s.T; t += gridDim.x * blockDim.x) {
     int st = s.t_status[t];
     bool allocated = (st & kAllocatedStatuses) != 0;
     if (!allocated && st != KAI_POD_PENDING) continue;
     int j = s.t_job[t];
     bool preemptible = (s.j_flags[j] & KAI_JOB_PREEMPTIBLE) != 0;
+    if (s.j_queue[j] >= 0)  // every queue sum adds a subset of these summands
+      for (int r = 0; r < QR; r++) note_summand(s.t_req[(size_t)t * s.R + r], r, mag[r], inexact);
     for (int q = s.j_queue[j]; q >= 0; q = s.q_parent[q])
       for (int r = 0; r < QR; r++) {
         double v = s.t_req[(size_t)t * s.R + r];
@@ -92,6 +190,38 @@ __global__ void k_queue_usage(DevSnap s) {
           if (!preemptible) atomicAdd(&s.q_alloc_np[(size_t)r * s.Q + q], v);
         }
       }
+  }
+  open_sums_publish(s.osum, 1, mag, inexact, false);
+}
+
+// Runs after k_queue_usage: one warp per (resource, queue) of a resource whose sums could round redoes that queue's
+// Request / Allocated / AllocatedNonPreemptible in the oracle's order (job, podset, task = the caller's task index
+// order).  q_tasks lists the tasks under each queue in that order, so the work is O(T * depth) per resource.
+__global__ void k_queue_usage_ordered(DevSnap s) {
+  __shared__ double buf[8][3][kOrdChunk];
+  const int warp = threadIdx.x >> 5;
+  const int item = blockIdx.x * (blockDim.x >> 5) + warp;
+  if (warp >= 8 || item >= QR * s.Q) return;
+  const int r = item / s.Q, q = item % s.Q;
+  if (sums_exact(s.osum, 1, r)) return;
+  const int *list = s.q_tasks + s.q_task_begin[q];
+  double out[3];
+  warp_ordered_sums<3>(s.q_task_begin[q + 1] - s.q_task_begin[q], [&](int k, double *v) {
+    const int t = list[k];
+    const int st = s.t_status[t];
+    const bool allocated = (st & kAllocatedStatuses) != 0;
+    if (!allocated && st != KAI_POD_PENDING) return;
+    const double x = s.t_req[(size_t)t * s.R + r];
+    v[0] = x;
+    if (allocated) {
+      v[1] = x;
+      if (!(s.j_flags[s.t_job[t]] & KAI_JOB_PREEMPTIBLE)) v[2] = x;
+    }
+  }, buf[warp], out);
+  if ((threadIdx.x & 31) == 0) {
+    s.q_request[(size_t)r * s.Q + q] = out[0];
+    s.q_alloc[(size_t)r * s.Q + q] = out[1];
+    s.q_alloc_np[(size_t)r * s.Q + q] = out[2];
   }
 }
 

@@ -67,6 +67,26 @@ def main():
                     and np.array_equal(res.node_releasing[:, own], ref.node_releasing[:, own]))
             print(f"rank {rank}/{world} cycle {kw} {action}: {'OK' if same else 'MISMATCH'} placed {res.pods_placed} evicted {res.pods_evicted}", flush=True)
             ok = ok and same
+    # non-round values (tests/value_regime.py): inexact node totals and queue sums must give every rank the oracle's bits
+    import value_regime as vr
+    for name in ("a_totals", "b_queues"):
+        snap, _ = vr.regime(name)  # both regimes run with the default configuration
+        eng.load(snap)
+        res = eng.run("allocate")
+        o = Oracle()
+        o.load(snap)
+        ref = o.run("allocate")
+        own = engine.shard_node_mask(snap.node_name_rank, world, rank)
+        same = (np.array_equal(res.task_node, ref.task_node) and np.array_equal(res.task_status, ref.task_status)
+                and np.array_equal(res.visits, ref.visits) and np.array_equal(res.total_resource, ref.total_resource)
+                and np.array_equal(res.queue_request, ref.queue_request)
+                and np.array_equal(res.queue_allocated, ref.queue_allocated)
+                and np.array_equal(res.queue_allocated_non_preemptible, ref.queue_allocated_non_preemptible)
+                and np.array_equal(res.queue_fair_share, ref.queue_fair_share)
+                and np.array_equal(res.node_idle[:, own], ref.node_idle[:, own]))
+        print(f"rank {rank}/{world} value regime {name}: {'OK' if same else 'MISMATCH'} placed {res.pods_placed}", flush=True)
+        ok = ok and same
+        o.close()
     # topology-constrained gangs (config-4 shape) on node-striped GPUs
     for kw in (dict(n_nodes=512, n_gangs=60, nodes_per_rack=8, racks_per_leaf=4, leaves_per_spine=4, running_fraction=0.3),
                dict(n_nodes=2048, n_gangs=300)):

@@ -1,7 +1,10 @@
 """Parity of the CUDA engine with the CPU oracle through the C ABI (GPU box only).
 
 Bit-exact: bindings (task -> node), task statuses, job visiting order and outcomes, node Idle/Releasing
-tables, queue Allocated / fair-share tables (DRF inputs; tolerance 0 here since inputs are integer valued).
+tables, queue Allocated / Request / totals.  Fair shares are compared within 1e-6 here; the inputs of this module are
+integer valued, so every sum is exact in any order and these tests cannot tell a summation order from another.
+test_value_regime_gpu.py runs non-round values (inexact totals and queue sums, score near-ties, fractional fair shares)
+with every table, the fair shares included, compared bit for bit.
 """
 import os
 
