@@ -187,34 +187,36 @@ struct Cand {
   uint32_t rank;
   int ln;
 };
-__device__ __forceinline__ bool better(double sa, uint32_t ra, double sb, uint32_t rb) {
+// better / binpack_score / node_key are compiled for the host too: the solver answers small restricted sweeps from its
+// node mirror with the very operations the scanners run (kadd & co. are IEEE binary64 without contraction on both sides)
+KAI_HD __forceinline__ bool better(double sa, uint32_t ra, double sb, uint32_t rb) {
   if (ra == kRankNone) return false;
   if (rb == kRankNone) return true;
   return sa > sb || (sa == sb && ra < rb);
 }
 
 // pack.go:45-64
-__device__ __forceinline__ double binpack_score(double mn, double mx, double cur, double overall) {
+KAI_HD __forceinline__ double binpack_score(double mn, double mx, double cur, double overall) {
   if (overall == 0) return 0.0;
   if (mx == 0) return 0.0;
   if (mn == mx) return 9.0;
-  double t1 = __dsub_rn(cur, mn);
-  double t2 = __dsub_rn(mx, mn);
-  double t3 = __ddiv_rn(t1, t2);
-  double t4 = __dsub_rn(1.0, t3);
-  return __dmul_rn(9.0, t4);
+  double t1 = ksub(cur, mn);
+  double t2 = ksub(mx, mn);
+  double t3 = kdiv(t1, t2);
+  double t4 = ksub(1.0, t3);
+  return kmul(9.0, t4);
 }
 
 // FittingNode (session.go:201-232) + NodeOrderFn sum (session_plugins.go:427-437) of one node row given as
 // Idle/Releasing vectors.  Returns false if the node does not fit; fit_i = fits on Idle alone.
-__device__ __forceinline__ bool node_key(const Decision &d, int R, const double *I, const double *L, int stride,
-                                         double a_gpu, double a_cpu, double gpu_count, uint32_t nflags, int n,
-                                         double &score, bool &fit_i) {
+KAI_HD __forceinline__ bool node_key(const Decision &d, int R, const double *I, const double *L, int stride,
+                                     double a_gpu, double a_cpu, double gpu_count, uint32_t nflags, int n,
+                                     double &score, bool &fit_i) {
   bool fit_ri = true;
   fit_i = true;
   for (int r = 0; r < R; r++) {
     double i = I[r * stride];
-    double avail = __dadd_rn(i, L[r * stride]);
+    double avail = kadd(i, L[r * stride]);
     double rq = d.req[r];
     if (r >= 3) {
       if (rq != 0 && rq > avail) fit_ri = false;
@@ -226,21 +228,21 @@ __device__ __forceinline__ bool node_key(const Decision &d, int R, const double 
   }
   if (!fit_ri) return false;
   score = 0.0;
-  score = __dadd_rn(score, (d.best_effort || fit_i) ? 100.0 : 0.0);  // nodeavailability.go:29-40
-  score = __dadd_rn(score, 0.0);                                     // gpusharingorder (whole GPUs)
+  score = kadd(score, (d.best_effort || fit_i) ? 100.0 : 0.0);  // nodeavailability.go:29-40
+  score = kadd(score, 0.0);                                   // gpusharingorder (whole GPUs)
   bool cpu_only_node = !(nflags & KAI_NODE_NOT_CPU_ONLY) && a_gpu <= 0;
-  score = __dadd_rn(score, (!d.gpu_task && cpu_only_node) ? 10.0 : 0.0);  // resourcetype.go:29-41
-  score = __dadd_rn(score, (d.nominated == n) ? 1000000.0 : 0.0);        // nominatednode.go:29-41
-  double cur = __dadd_rn(I[d.res * stride], L[d.res * stride]);
+  score = kadd(score, (!d.gpu_task && cpu_only_node) ? 10.0 : 0.0);  // resourcetype.go:29-41
+  score = kadd(score, (d.nominated == n) ? 1000000.0 : 0.0);        // nominatednode.go:29-41
+  double cur = kadd(I[d.res * stride], L[d.res * stride]);
   double overall = d.res == KAI_RES_GPU ? a_gpu : a_cpu;
   double place;
   if (d.strategy == KAI_PLACEMENT_BINPACK) {
     place = binpack_score(d.mn, d.mx, cur, overall);
   } else {  // spread.go:16-36
     double cnt = d.res == KAI_RES_GPU ? (double)(long long)gpu_count : overall;
-    place = cnt == 0 ? 0.0 : __ddiv_rn(cur, cnt);
+    place = cnt == 0 ? 0.0 : kdiv(cur, cnt);
   }
-  score = __dadd_rn(score, place);
+  score = kadd(score, place);
   return true;
 }
 

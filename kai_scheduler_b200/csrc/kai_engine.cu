@@ -1116,6 +1116,7 @@ static bool engine_launch_record(void *ctx, const LaunchRec &rec) {
 int kai_engine_run(kai_engine *e, kai_action action, kai_result *out) {
   if (!e || !out) return KAI_ERR_INVALID;
   if (!e->loaded) return e->fail(KAI_ERR_STATE, "no snapshot loaded");
+  const double t_entry = HostBackend::now();  // KAI_PROFILE: the solver's set-up split
   const bool solver_action = action == KAI_ACTION_RECLAIM || action == KAI_ACTION_CONSOLIDATION || action == KAI_ACTION_PREEMPT ||
                              action == KAI_ACTION_STALEGANGEVICTION;
   if (action != KAI_ACTION_ALLOCATE && !solver_action) return e->fail(KAI_ERR_UNSUPPORTED, "unknown action");
@@ -1278,6 +1279,7 @@ int kai_engine_run(kai_engine *e, kai_action action, kai_result *out) {
     hb.gang_fast = getenv("KAI_NO_GANG_FAST") == nullptr;
     hb.gang_bulk = hb.gang_replayed = hb.gang_failed = 0;
     hb.rank_to_node = e->rank_to_node_h.data();
+    const double t_mirror0 = HostBackend::now();
     CK(cudaEventSynchronize(e->ev_mirror));
     if (refresh_mirror && !e->h_tmp.empty()) {  // re-read tables -> node-major mirror
       for (int n = 0; n < e->N; n++)
@@ -1287,6 +1289,7 @@ int kai_engine_run(kai_engine *e, kai_action action, kai_result *out) {
         }
     }
     if (feed_mirror) e->mirror_valid = true;  // from here on the host-sequenced deltas keep it in step
+    const double t_mirror1 = HostBackend::now();
     // ---- sequencer state on the host ----
     const DevSnap &hs = e->hs;
     const int Q = e->Q, J = e->J;
@@ -1367,7 +1370,7 @@ int kai_engine_run(kai_engine *e, kai_action action, kai_result *out) {
     ctl.dec.task = -1;
     ctl.ctx_job = ctl.ctx_ps = -1;
     ctl.seq = p.seq0;
-    long long solver_scenarios = 0, solver_topk = 0;
+    long long solver_scenarios = 0, solver_topk = 0, solver_host_sweeps = 0, solver_host_topk = 0;
     if (!solver_action) {
       hb.run_allocate();
     } else {
@@ -1376,6 +1379,7 @@ int kai_engine_run(kai_engine *e, kai_action action, kai_result *out) {
         e->on_other_node.assign(T, -1);
         e->on_other_status.assign(T, 0);
       }
+      const double t_slots = HostBackend::now();
       std::vector<int> n0(T), s0(T);
       for (int t = 0; t < T; t++) {
         bool on = (hs.t_status[t] & kActiveUsed) && hs.t_node[t] >= 0;
@@ -1391,6 +1395,7 @@ int kai_engine_run(kai_engine *e, kai_action action, kai_result *out) {
       solver.j_last_start = e->j_last_start.empty() ? nullptr : e->j_last_start.data();
       solver.j_stale_since = e->j_stale_since.empty() ? nullptr : e->j_stale_since.data();
       solver.now_s = e->now_s;
+      const double t_ctor = HostBackend::now();
       if (action == KAI_ACTION_RECLAIM)
         solver.run_reclaim();
       else if (action == KAI_ACTION_PREEMPT)
@@ -1400,15 +1405,21 @@ int kai_engine_run(kai_engine *e, kai_action action, kai_result *out) {
       else
         solver.run_consolidation();
       hb.publish(DK_DONE);
-      hb.t_total = HostBackend::now() - t_begin;
+      const double t_end = HostBackend::now();
+      hb.t_total = t_end - t_begin;
       if (getenv("KAI_PROFILE"))
         fprintf(stderr, "[kai] solver host profile: %lld simulations; sweeps %.1f ms, simulation set-up %.1f ms, evicting recorded victims %.1f ms, victims queues %.1f ms\n",
                 solver.simulations, solver.t_sweeps * 1e3, solver.t_sim_setup * 1e3, solver.t_evict * 1e3, solver.t_victims_queue * 1e3);
       if (getenv("KAI_PROFILE"))
         fprintf(stderr, "[kai] solver host profile: scenario loop: victims pop %.1f ms, tasks_to_evict %.1f, add potential %.1f, filter %.1f, filter init (top-k sweep) %.1f, by-pod solve %.1f\n",
                 solver.t_vq_pop * 1e3, solver.t_tte * 1e3, solver.t_addp * 1e3, solver.t_filter * 1e3, solver.t_finit * 1e3, solver.t_bypod * 1e3);
+      if (getenv("KAI_PROFILE"))
+        fprintf(stderr, "[kai] solver host profile: victims queues: %lld built (leaf tops %.2f ms), %lld copied (%.2f ms)\n",
+                solver.n_vq_build, solver.t_vq_top * 1e3, solver.n_vq_copy, solver.t_vq_copy * 1e3);
       solver_scenarios = solver.scenarios;
       solver_topk = solver.topk_sweeps;
+      solver_host_sweeps = solver.host_sweeps;
+      solver_host_topk = solver.host_topks;
       // one status per task for the allocate path: the entry on the task's current node; the other entry persists
       for (auto &x : e->on_extra) {  // the entry on the task's current node belongs in slot 0
         const int t = x[0], cur = hs.t_node[t];
@@ -1442,13 +1453,20 @@ int kai_engine_run(kai_engine *e, kai_action action, kai_result *out) {
           }
         }
       }
+      if (getenv("KAI_PROFILE"))
+        fprintf(stderr, "[kai] solver set-up / teardown: kai_engine_run entry to solver start %.2f ms (before the mirror wait %.2f, "
+                "mirror wait + refresh %.2f, task slots %.2f, Solver construction %.2f, prepare() %.2f); solver end to the "
+                "action's end event %.2f ms\n",
+                (t_ctor - t_entry) * 1e3 + solver.t_prepare * 1e3, (t_mirror0 - t_entry) * 1e3, (t_mirror1 - t_mirror0) * 1e3,
+                (t_begin - t_slots) * 1e3, (t_ctor - t_begin) * 1e3, solver.t_prepare * 1e3, (HostBackend::now() - t_end) * 1e3);
     }
     if (launch_mode) cudaEventRecord(e->ev[3], e->stream);  // after the DONE launch: the action's span on the device
     CK(cudaStreamSynchronize(e->stream));
     if (launch_mode) CK(cudaGetLastError());
     if (solver_action && getenv("KAI_PROFILE"))
-      fprintf(stderr, "[kai] solver: %lld scenarios simulated, %lld node sweeps, %lld top-k sweeps, %lld minmax exchanges\n",
-              solver_scenarios, seq.sweeps, solver_topk, seq.minmax_exchanges);
+      fprintf(stderr, "[kai] solver: %lld scenarios simulated, %lld node sweeps, %lld top-k sweeps, %lld minmax exchanges, "
+              "%lld restricted sweeps and %lld top-k lists answered on the host\n",
+              solver_scenarios, seq.sweeps, solver_topk, seq.minmax_exchanges, solver_host_sweeps, solver_host_topk);
     {
       long long cd[48];
       CK(cudaMemcpy(cd, e->counters, sizeof(cd), cudaMemcpyDeviceToHost));
@@ -1547,6 +1565,7 @@ int kai_engine_run(kai_engine *e, kai_action action, kai_result *out) {
     return e->fail(KAI_ERR_CUDA, m2);
   }
   if (c[6] == 2) return e->fail(KAI_ERR_UNSUPPORTED, "topology: more preferred-level domains than the score table holds (kDomBuckets)");
+  if (c[6] == Solver::kSeqErrHostSweep) return e->fail(KAI_ERR_INVALID, e->hb.error_msg);
   if (c[6] != 0) return e->fail(KAI_ERR_CUDA, "device sequencer overflow (statement log)");
   return download(e, out, c[0], c[3], c[4]);
 }

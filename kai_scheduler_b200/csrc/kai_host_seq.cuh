@@ -35,6 +35,7 @@ struct HostBackend {
   int batching = 1;
   double timeout_s = 20.0;
   bool failed = false;
+  char error_msg[256] = {0};  // why the action failed, when the sequencer sets Seq::error to a code that carries a message
   const int *rank_to_node = nullptr;  // host copy
   Ctl ctl;
   Seq seq;

@@ -8,7 +8,8 @@
 // Division of work (same as allocate): everything that is O(nodes) runs on the GPU —
 //   * every allocateTask of every simulation is one restricted, pipeline-only sweep of the scanners' tiles
 //     (DK_SCAN with XB_RESTRICT: fit on Idle+Releasing, NodeOrderFn score, argmax on (score, name rank)),
-//     preceded by the binpack min/max exchange over the same node set (DK_MINMAX);
+//     preceded by the binpack min/max exchange over the same node set (DK_MINMAX) — or, when that set is small, the
+//     same computation on the host mirror (host_sweep);
 //   * the feasible-node set of a job (FeasibleNodesForJob) is a per-row bit the scanners compute from their tiles
 //     (XB_SNAP_*), later edited by ND_FEAS_SET/CLR deltas when victims' nodes join the set;
 //   * the idle-GPU scenario filter's "k nodes with most idle+releasing GPUs" is a DK_TOPK sweep;
@@ -109,6 +110,8 @@ struct Solver {
   std::vector<SOp> ops;
 
   long long sweeps = 0, scenarios = 0, topk_sweeps = 0, simulations = 0;
+  double t_vq_copy = 0, t_vq_top = 0, t_prep_split[3] = {0, 0, 0};
+  long long n_vq_copy = 0, n_vq_build = 0;
   double t_sweeps = 0, t_sim_setup = 0, t_evict = 0, t_victims_queue = 0, t_vq_pop = 0, t_tte = 0, t_addp = 0, t_filter = 0, t_bypod = 0, t_finit = 0;
 
   Solver(HostBackend &hb_, std::vector<int> &n0, std::vector<int> &s0, std::vector<int> &n1, std::vector<int> &s1,
@@ -123,6 +126,12 @@ struct Solver {
     touched_epoch.assign(N, -1);
     startIg.assign(N, 0);
     startLg.assign(N, 0);
+    // Host answers need the mirror of every node and no topology term; with several GPUs every rank would answer alike,
+    // but the multi-GPU path keeps its MINMAX exchange (DESIGN.md §7).
+    const char *mx = getenv("KAI_HOST_SWEEP_MAX");
+    host_sweep_max = mx ? atoi(mx) : kHostSweepMaxDefault;
+    if (cfg.shard_count > 1 || seq.topology || !seq.mirror) host_sweep_max = 0;
+    host_sweep_check = getenv("KAI_HOST_SWEEP_CHECK") != nullptr;
   }
 
   // ---------------- small accessors ----------------
@@ -143,6 +152,7 @@ struct Solver {
     return st[t] == KAI_POD_PENDING || (!real && st[t] == KAI_POD_RELEASING && tvirt[t]);
   }
   int count_ps(int ps, int mask) const {
+    if (mask == kActiveAllocated) return ps_active[ps];
     int c = 0;
     for (int t = pst_begin(ps); t < pst_end(ps); t++)
       if (st[t] & mask) c++;
@@ -336,6 +346,24 @@ struct Solver {
     const double before = Ig(n) + Lg(n);
     emit_delta(seq, n, code, t);  // also applies the delta to the mirror (seq.mirror)
     if (s.nflags[n] & KAI_NODE_READY) free_ready += (Ig(n) + Lg(n)) - before;
+    if (host_sweep_max > 0) gpu_free_update(n);
+  }
+  // nodes with idle or releasing GPUs right now (the XB_SNAP_GPUFREE definition), kept as the mirror changes, so that an
+  // attempt's base feasible set is a copy of a short list rather than a scan of every node
+  std::vector<int> gpu_free_list, gpu_free_pos;
+  void gpu_free_update(int n) {
+    const bool in = Ig(n) > 0 || Lg(n) > 0;
+    if (in == (gpu_free_pos[n] >= 0)) return;
+    if (in) {
+      gpu_free_pos[n] = (int)gpu_free_list.size();
+      gpu_free_list.push_back(n);
+    } else {
+      const int i = gpu_free_pos[n], last = gpu_free_list.back();
+      gpu_free_list[i] = last;
+      gpu_free_pos[last] = i;
+      gpu_free_list.pop_back();
+      gpu_free_pos[n] = -1;
+    }
   }
   void node_add_task(int t) {  // node_info.go:457-493 with the task's current status
     int n = tn[t], status = st[t];
@@ -363,6 +391,9 @@ struct Solver {
   // jobs with Pending tasks (utils.GetAllPendingJobs, actions/utils/action.go:122-130), kept as statuses change
   std::vector<int> pending_cnt;
   std::set<int> pending_jobs;
+  // tasks with an active-allocated status per podset (count_ps(ps, kActiveAllocated)), kept by set_status: the
+  // victims queues ask it of every job of every leaf queue
+  std::vector<int> ps_active;
   void set_status(int t, int status) {
     const int j = tjob(t);
     if (st[t] == KAI_POD_PENDING && status != KAI_POD_PENDING) {
@@ -370,6 +401,8 @@ struct Solver {
     } else if (st[t] != KAI_POD_PENDING && status == KAI_POD_PENDING) {
       if (pending_cnt[j]++ == 0) pending_jobs.insert(j);
     }
+    const bool was_active = (st[t] & kActiveAllocated) != 0, is_active = (status & kActiveAllocated) != 0;
+    if (was_active != is_active) ps_active[s.t_podset[t]] += is_active ? 1 : -1;
     st[t] = status;
     job_cache[j].tta_valid = job_cache[j].res_valid = false;
     if (s.j_queue[j] >= 0) leaf_epoch[s.j_queue[j]]++;
@@ -520,7 +553,7 @@ struct Solver {
   }
 
   // ---------------- GPU sweeps ----------------
-  bool gpu_failed() const { return hb.failed; }
+  bool gpu_failed() const { return hb.failed || seq.error == kSeqErrHostSweep; }
   // allocateTask (allocate.go:121-163) in a simulation: one restricted pipeline-only sweep
   unsigned int sweep_extra_bits = 0;  // XB_RESTRICT_DOM while a topology domain is selected
   int sweep_pick_node(int t) {
@@ -542,14 +575,147 @@ struct Solver {
     // pack.go:66-86 over the node set of this simulation: the scanners exchange their extremes among themselves
     ctl.trk[0].dirty = ctl.trk[1].dirty = 1;
     const double t0 = HostBackend::now();
-    hb.sweep_single(sweep_extra_bits);  // only the winner is needed
+    const bool on_host = host_sweep_usable();
+    if (!on_host || host_sweep_check) {
+      hb.sweep_single(sweep_extra_bits);  // only the winner is needed
+      sweeps++;
+    }
+    if (on_host && !hb.failed) {
+      const Winner w = host_sweep();
+      if (host_sweep_check && !same_winner(w, ctl.win)) {
+        snprintf(hb.error_msg, sizeof(hb.error_msg),
+                 "KAI_HOST_SWEEP_CHECK: task %d: host sweep picked node %d (score bits %016llx, rank %u, flags %u), "
+                 "GPU sweep node %d (score bits %016llx, rank %u, flags %u)",
+                 t, w.node, (unsigned long long)kbits(w.score), w.rank, w.flags, ctl.win.node,
+                 (unsigned long long)kbits(ctl.win.score), ctl.win.rank, ctl.win.flags);
+        seq.error = kSeqErrHostSweep;
+      }
+      ctl.win = w;
+      host_sweeps++;
+    }
     t_sweeps += HostBackend::now() - t0;
-    sweeps++;
-    if (hb.failed) return -1;
+    if (gpu_failed()) return -1;
     return ctl.win.node;
+  }
+  // ---- restricted sweeps answered from the host mirror ----
+  // A simulation's feasible set (FeasibleNodesForJob) is the attempt's base set (nodes with idle or releasing GPUs when
+  // the attempt started) plus the victims' nodes.  When it holds at most host_sweep_max rows, the answer is computed here
+  // from seq.mirror in the scanners' order (extremes, predicate mask, node_key, argmax on score desc / name rank asc)
+  // instead of a GPU round trip.  No record is published: the queued node and feasible-set deltas stay queued for the
+  // next record, so the scanners' tiles stay in step, and no sequence number is consumed.
+  static constexpr int kHostSweepMaxDefault = 256;
+  static constexpr int kSeqErrHostSweep = 3;  // Seq::error: KAI_HOST_SWEEP_CHECK found a difference
+  int host_sweep_max = 0;         // KAI_HOST_SWEEP_MAX (0: every sweep runs on the GPU)
+  bool host_sweep_check = false;  // KAI_HOST_SWEEP_CHECK: run the GPU sweep as well and fail on any difference
+  long long host_sweeps = 0;
+  std::vector<int> base_list;  // the attempt's base feasible set (valid when base_known)
+  bool base_known = false;
+  bool host_sweep_usable() const {
+    return host_sweep_max > 0 && base_known && !feas_all && sweep_extra_bits == 0 &&
+           base_list.size() + feas_extra_list.size() <= (size_t)host_sweep_max;
+  }
+  static bool same_winner(const Winner &a, const Winner &b) {
+    return a.node == b.node && a.rank == b.rank && a.flags == b.flags && (a.node < 0 || kbits(a.score) == kbits(b.score));
+  }
+  Winner host_sweep() {
+    Decision d = ctl.dec;
+    const double *Ag = s.alloc + (size_t)KAI_RES_GPU * N, *Ac = s.alloc + (size_t)KAI_RES_CPU * N;
+    const int nb = (int)base_list.size(), ne = (int)feas_extra_list.size();
+    auto row_at = [&](int i) { return i < nb ? base_list[i] : feas_extra_list[i - nb]; };
+    if (d.strategy == KAI_PLACEMENT_BINPACK) {  // the fused min/max of the scanners (XB_FUSED_MM)
+      double mn = DBL_MAX, mx = 0;
+      const double *A = d.res == KAI_RES_GPU ? Ag : Ac;
+      for (int i = 0; i < nb + ne; i++) {
+        const int n = row_at(i);
+        if (A[n] == 0) continue;
+        const double *row = seq.mirror + (size_t)n * 2 * R;
+        const double cur = kadd(row[d.res], row[R + d.res]);
+        if (cur < mn) mn = cur;
+        if (cur > mx) mx = cur;
+      }
+      d.mn = mn;
+      d.mx = mx;
+    }
+    const uint32_t *mask = d.pred_class >= 0 ? s.pred_mask + (size_t)d.pred_class * s.mask_words : nullptr;
+    double bs = -1.0;
+    uint32_t brank = kRankNone;
+    int bnode = -1;
+    bool bfit_i = false;
+    for (int i = 0; i < nb + ne; i++) {
+      const int n = row_at(i);
+      if (mask && !((mask[n >> 5] >> (n & 31)) & 1u)) continue;
+      const double *row = seq.mirror + (size_t)n * 2 * R;
+      double score;
+      bool fit_i;
+      if (!node_key(d, R, row, row + R, 1, Ag[n], Ac[n], s.gpu_count[n], s.nflags[n], n, score, fit_i)) continue;
+      const uint32_t rk = (uint32_t)s.name_rank[n];
+      if (better(score, rk, bs, brank)) {
+        bs = score;
+        brank = rk;
+        bnode = n;
+        bfit_i = fit_i;
+      }
+    }
+    Winner w;
+    w.score = bs;
+    w.rank = brank;
+    w.node = bnode;
+    // publish_candidate's flags; the trackers are dirty (no event bits) and nothing is batched
+    w.flags = (bnode >= 0 && !d.pipeline_only && (d.best_effort || bfit_i)) ? SLOT_TO_IDLE : 0u;
+    return w;
   }
   // the k rows with most idle + releasing GPUs (values, descending); pages of top-M lists until k are known
   std::vector<std::pair<double, int>> sweep_topk_idle(int k, unsigned int snap_bits) {
+    std::vector<std::pair<double, int>> host;
+    if (host_sweep_max > 0 && host_topk(k, host)) {
+      if (!host_sweep_check) {
+        if (snap_bits) {  // the feasible-set snapshot still reaches the scanners, without a round trip
+          ctl.xbits = snap_bits;
+          hb.flush_deltas();
+          ctl.xbits = 0;
+        }
+        host_topks++;
+        return host;
+      }
+      std::vector<std::pair<double, int>> dev = sweep_topk_idle_gpu(k, snap_bits);
+      if (!hb.failed && dev != host) {
+        snprintf(hb.error_msg, sizeof(hb.error_msg),
+                 "KAI_HOST_SWEEP_CHECK: top-%d idle-GPU rows differ: host %zu rows (first node %d), GPU %zu rows (first node %d)",
+                 k, host.size(), host.empty() ? -1 : host[0].second, dev.size(), dev.empty() ? -1 : dev[0].second);
+        seq.error = kSeqErrHostSweep;
+      }
+      host_topks++;
+      return host;
+    }
+    return sweep_topk_idle_gpu(k, snap_bits);
+  }
+  // The same k rows from the mirror: every row with idle + releasing GPUs > 0 is in gpu_free_list; after them come the
+  // rows whose sum is exactly 0, in name-rank order (rows below 0 would follow: the GPU answers when they are needed).
+  long long host_topks = 0;
+  bool host_topk(int k, std::vector<std::pair<double, int>> &out) {
+    if (gpu_free_list.size() > (size_t)host_sweep_max) return false;
+    struct Row {
+      double key;
+      int rank, node;
+    };
+    std::vector<Row> pos;
+    for (int n : gpu_free_list) {
+      const double key = kadd(Ig(n), Lg(n));
+      if (key > 0) pos.push_back({key, s.name_rank[n], n});
+    }
+    std::sort(pos.begin(), pos.end(), [](const Row &a, const Row &b) { return a.key > b.key || (a.key == b.key && a.rank < b.rank); });
+    out.clear();
+    for (size_t i = 0; i < pos.size() && (int)out.size() < k; i++) out.push_back({pos[i].key, pos[i].node});
+    const int scan_cap = 4 * host_sweep_max + k;
+    for (int r = 0; r < N && (int)out.size() < k; r++) {
+      if (r >= scan_cap) return false;
+      const int n = hb.rank_to_node[r];
+      const double key = kadd(Ig(n), Lg(n));
+      if (key == 0) out.push_back({key, n});
+    }
+    return (int)out.size() == std::min(k, N);
+  }
+  std::vector<std::pair<double, int>> sweep_topk_idle_gpu(int k, unsigned int snap_bits) {
     std::vector<std::pair<double, int>> out;
     Decision &d = ctl.dec;
     d.restricted = 0;
@@ -1458,6 +1624,7 @@ struct Solver {
   }
   int victim_leaf_top(JobsOrder &jo, int q) {
     if (vq_top_epoch[q] == leaf_epoch[q]) return vq_top[q];
+    const double tt = HostBackend::now();
     int best = -1;
     unsigned long long best_key = 0;
     for (int i = s.q_job_begin[q]; i < s.q_job_begin[q + 1]; i++) {
@@ -1471,6 +1638,7 @@ struct Solver {
     }
     vq_top[q] = best;
     vq_top_epoch[q] = leaf_epoch[q];
+    t_vq_top += HostBackend::now() - tt;
     return best;
   }
   const std::vector<int> &victim_leaf_list(JobsOrder &jo, int q) {
@@ -1530,9 +1698,13 @@ struct Solver {
   void build_victims_queue(JobsOrder &jo, int pending_job) {
     if (vq_proto_job == pending_job && vq_proto_kind == solver_kind && vq_proto_commit == commit_epoch && ops.empty() &&
         !getenv("KAI_NO_VICTIM_CACHE")) {
+      const double tc = HostBackend::now();
       jo.copy_from(vq_proto);
+      t_vq_copy += HostBackend::now() - tc;
+      n_vq_copy++;
       return;
     }
+    n_vq_build++;
     jo.init(this, true);
     if (build_victims_queue_cached(jo, pending_job)) {
       vq_proto.copy_from(jo);
@@ -1702,6 +1874,9 @@ struct Solver {
         if (!(req(t, KAI_RES_GPU) > 0)) feas_all = true;
     pending_snap_bits = feas_all ? XB_SNAP_ALL : XB_SNAP_GPUFREE;
     views.clear();
+    // No node changes before that TOPK record, so the rows it will flag are the GPU-free rows of now (= in_base()).
+    base_known = host_sweep_max > 0 && !feas_all && gpu_free_list.size() <= (size_t)host_sweep_max;
+    if (base_known) base_list = gpu_free_list;
   }
 
   // ---------------- minimal_job_comparison.go ----------------
@@ -1754,7 +1929,9 @@ struct Solver {
     m[job_signature[j]] = j;
   }
 
+  double t_prepare = 0;
   void prepare() {
+    const double t0 = HostBackend::now();
     job_cache.assign(J, Cache());
     vq_leaf.assign(Q, {});
     vq_leaf_epoch.assign(Q, -1);
@@ -1763,13 +1940,22 @@ struct Solver {
     leaf_epoch.assign(Q, 0);
     pending_cnt.assign(J, 0);
     pending_jobs.clear();
-    for (int t = 0; t < T; t++)
+    ps_active.assign(S, 0);
+    for (int t = 0; t < T; t++) {
       if (st[t] == KAI_POD_PENDING && pending_cnt[tjob(t)]++ == 0) pending_jobs.insert(tjob(t));
+      if (st[t] & kActiveAllocated) ps_active[s.t_podset[t]]++;
+    }
     feas_extra.assign(N, 0);
     ops_truncate(0);
     free_ready = 0;  // once per action, from the mirror of the GPU column the action starts with
-    for (int n = 0; n < N; n++)
+    base_known = false;
+    gpu_free_list.clear();
+    if (host_sweep_max > 0) gpu_free_pos.assign(N, -1);
+    for (int n = 0; n < N; n++) {
       if (s.nflags[n] & KAI_NODE_READY) free_ready += Ig(n) + Lg(n);
+      if (host_sweep_max > 0) gpu_free_update(n);
+    }
+    t_prepare += HostBackend::now() - t0;
   }
 
   // ---------------- actions/reclaim/reclaim.go:46-119 ----------------
