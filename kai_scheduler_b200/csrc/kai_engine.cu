@@ -149,6 +149,7 @@ struct kai_engine {
   // solver actions: second NodeInfo.PodInfos entry of a task (evicted from A, pipelined to B), mirror of the GPU column
   std::vector<int> on_other_node, on_other_status;
   std::vector<std::array<int, 3>> on_extra;  // (task, node, status) node entries beyond two per task (kai_solver.cuh)
+  SolverScratch solver_scratch;              // the solver's per-node / per-job / per-task scratch (sized at first use)
   std::vector<double> h_mirror;  // host mirror of Idle / Releasing, node-major [N][2][R]
   std::vector<double> h_tmp;     // staging for the re-read after a device-sequenced action
   int *d_node_domain = nullptr;
@@ -1379,15 +1380,8 @@ int kai_engine_run(kai_engine *e, kai_action action, kai_result *out) {
         e->on_other_node.assign(T, -1);
         e->on_other_status.assign(T, 0);
       }
-      const double t_slots = HostBackend::now();
-      std::vector<int> n0(T), s0(T);
-      for (int t = 0; t < T; t++) {
-        bool on = (hs.t_status[t] & kActiveUsed) && hs.t_node[t] >= 0;
-        n0[t] = on ? hs.t_node[t] : -1;
-        s0[t] = hs.t_node_status[t];
-      }
       double t_begin = HostBackend::now();
-      Solver solver(hb, n0, s0, e->on_other_node, e->on_other_status, e->on_extra);
+      Solver solver(hb, e->solver_scratch, e->on_other_node, e->on_other_status, e->on_extra);
       solver.use_signatures = e->cfg.use_scheduling_signatures != 0;
       solver.job_signature = e->job_signature.empty() ? nullptr : e->job_signature.data();
       solver.q_preempt_mrt = e->q_preempt_mrt.empty() ? nullptr : e->q_preempt_mrt.data();
@@ -1420,9 +1414,15 @@ int kai_engine_run(kai_engine *e, kai_action action, kai_result *out) {
       solver_topk = solver.topk_sweeps;
       solver_host_sweeps = solver.host_sweeps;
       solver_host_topk = solver.host_topks;
-      // one status per task for the allocate path: the entry on the task's current node; the other entry persists
+      // one status per task for the allocate path: the entry on the task's current node; the other entry persists.
+      // Only tasks the action changed (slot_list) and tasks with entries beyond two slots can need it: for any other
+      // task slot 0 is the snapshot's, on its current node with its current node status.
+      const double t_teardown = HostBackend::now();
+      SolverScratch &scr = e->solver_scratch;
+      std::vector<int> &n0 = scr.n0, &s0 = scr.s0;
       for (auto &x : e->on_extra) {  // the entry on the task's current node belongs in slot 0
         const int t = x[0], cur = hs.t_node[t];
+        solver.take_slot(t);
         if (x[1] == cur && n0[t] != cur && e->on_other_node[t] != cur) {
           if (n0[t] < 0) {
             n0[t] = x[1];
@@ -1436,7 +1436,8 @@ int kai_engine_run(kai_engine *e, kai_action action, kai_result *out) {
       }
       e->on_extra.erase(std::remove_if(e->on_extra.begin(), e->on_extra.end(), [](const std::array<int, 3> &x) { return x[0] < 0; }),
                         e->on_extra.end());
-      for (int t = 0; t < T; t++) {
+      std::sort(scr.slot_list.begin(), scr.slot_list.end());  // ascending task order, as a scan of every task
+      for (int t : scr.slot_list) {
         int cur = hs.t_node[t];
         if (n0[t] >= 0 && n0[t] != cur && e->on_other_node[t] == cur) {
           std::swap(n0[t], e->on_other_node[t]);
@@ -1455,10 +1456,11 @@ int kai_engine_run(kai_engine *e, kai_action action, kai_result *out) {
       }
       if (getenv("KAI_PROFILE"))
         fprintf(stderr, "[kai] solver set-up / teardown: kai_engine_run entry to solver start %.2f ms (before the mirror wait %.2f, "
-                "mirror wait + refresh %.2f, task slots %.2f, Solver construction %.2f, prepare() %.2f); solver end to the "
-                "action's end event %.2f ms\n",
+                "mirror wait + refresh %.2f, sequencer state %.2f, Solver construction + scratch %.2f, prepare() %.2f); solver end "
+                "to the action's end event %.2f ms (task-slot reconciliation over %zu tasks %.2f)\n",
                 (t_ctor - t_entry) * 1e3 + solver.t_prepare * 1e3, (t_mirror0 - t_entry) * 1e3, (t_mirror1 - t_mirror0) * 1e3,
-                (t_begin - t_slots) * 1e3, (t_ctor - t_begin) * 1e3, solver.t_prepare * 1e3, (HostBackend::now() - t_end) * 1e3);
+                (t_begin - t_mirror1) * 1e3, (t_ctor - t_begin) * 1e3, solver.t_prepare * 1e3, (HostBackend::now() - t_end) * 1e3,
+                scr.slot_list.size(), (HostBackend::now() - t_teardown) * 1e3);
     }
     if (launch_mode) cudaEventRecord(e->ev[3], e->stream);  // after the DONE launch: the action's span on the device
     CK(cudaStreamSynchronize(e->stream));

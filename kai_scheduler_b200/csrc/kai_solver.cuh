@@ -21,7 +21,6 @@
 #include <array>
 #include <algorithm>
 #include <cmath>
-#include <functional>
 #include <map>
 #include <set>
 #include <vector>
@@ -30,14 +29,11 @@
 
 namespace kai {
 
-template <class T>
-struct HeapGo {  // container/heap (Go): same sift order, so non-antisymmetric comparators pop in the same order
-  std::vector<T> a;
-  std::function<bool(const T &, const T &)> less;
-  bool empty() const { return a.empty(); }
-  int len() const { return (int)a.size(); }
-  const T &peek() const { return a[0]; }
-  void up(int j) {
+// container/heap (Go) on a[0..n): the same sift sequence, so non-antisymmetric comparators pop in the same order.
+// The storage belongs to the caller (JobsOrder keeps every heap of a tree in one arena); `less` is any callable.
+struct HeapGo {
+  template <class Less>
+  static void up(int *a, int j, const Less &less) {
     for (;;) {
       int i = (j - 1) / 2;
       if (i == j || j <= 0 || !less(a[j], a[i])) break;
@@ -45,7 +41,8 @@ struct HeapGo {  // container/heap (Go): same sift order, so non-antisymmetric c
       j = i;
     }
   }
-  bool down(int i0, int n) {
+  template <class Less>
+  static bool down(int *a, int i0, int n, const Less &less) {
     int i = i0;
     for (;;) {
       int j1 = 2 * i + 1;
@@ -58,20 +55,90 @@ struct HeapGo {  // container/heap (Go): same sift order, so non-antisymmetric c
     }
     return i > i0;
   }
-  void push(const T &x) {
-    a.push_back(x);
-    up((int)a.size() - 1);
+  template <class Less>
+  static void push(int *a, int &n, int x, const Less &less) {  // a has room for n + 1 entries
+    a[n] = x;
+    up(a, n, less);
+    n++;
   }
-  T pop() {
-    int n = (int)a.size() - 1;
-    std::swap(a[0], a[n]);
-    down(0, n);
-    T x = a.back();
-    a.pop_back();
-    return x;
+  template <class Less>
+  static int pop(int *a, int &n, const Less &less) {
+    const int m = n - 1;
+    std::swap(a[0], a[m]);
+    down(a, 0, m, less);
+    n = m;
+    return a[m];
   }
-  void fix(int i) {
-    if (!down(i, (int)a.size())) up(i);
+  template <class Less>
+  static void fix(int *a, int n, int i, const Less &less) {
+    if (!down(a, i, n, less)) up(a, i, less);
+  }
+};
+
+struct SolverJobCache {  // tasks_to_allocate / its resource sum of one job or view
+  bool tta_valid = false, res_valid = false;
+  unsigned stamp = 0;  // session jobs: valid while equal to SolverScratch::job_epoch
+  std::vector<int> tta;
+  double res[QR] = {0, 0, 0};
+};
+
+// Per-node, per-job and per-task scratch of the solver kept by the engine across actions.  It is sized to the snapshot
+// and invalidated by epoch stamps (an entry is live while its stamp equals the current epoch) rather than reassigned,
+// so an action's set-up and each partial job pay for what they touch, not O(N + J + T).
+struct SolverScratch {
+  int N = -1, J = -1, T = -1;
+  // attempt-start idle / releasing GPUs of the nodes touched since the attempt began
+  std::vector<unsigned> node_stamp;
+  std::vector<double> start_ig, start_lg;
+  unsigned node_epoch = 0;
+  std::vector<SolverJobCache> job_cache;  // live jobs (invalidated per action and on every status change)
+  unsigned job_epoch = 0;
+  // per task: the recorded victims of a partial job, the tasks an idle-GPU filter has accounted
+  std::vector<unsigned> rec_stamp, seen_stamp;
+  unsigned rec_epoch = 0, seen_epoch = 0;
+  // slot 0 of a task's NodeInfo.PodInfos entries (node, status) for the tasks the action changed (slot_list); the
+  // others' slot is still the snapshot's
+  std::vector<int> n0, s0, slot_list;
+  std::vector<unsigned> slot_stamp;
+  unsigned slot_epoch = 0;
+
+  void size_for(int n, int j, int t) {
+    if (n != N) {
+      node_stamp.assign(n, 0);
+      start_ig.assign(n, 0);
+      start_lg.assign(n, 0);
+      node_epoch = 0;
+      N = n;
+    }
+    if (j != J) {
+      job_cache.assign(j, SolverJobCache());
+      job_epoch = 0;
+      J = j;
+    }
+    if (t != T) {
+      rec_stamp.assign(t, 0);
+      seen_stamp.assign(t, 0);
+      n0.assign(t, -1);
+      s0.assign(t, 0);
+      slot_stamp.assign(t, 0);
+      rec_epoch = seen_epoch = slot_epoch = 0;
+      T = t;
+    }
+  }
+  template <class S>
+  static unsigned bump(unsigned &epoch, std::vector<S> &stamped, unsigned S::*field) {
+    if (++epoch == 0) {  // wrapped: no stale stamp may match the new epoch
+      for (S &x : stamped) x.*field = 0;
+      epoch = 1;
+    }
+    return epoch;
+  }
+  static unsigned bump(unsigned &epoch, std::vector<unsigned> &stamps) {
+    if (++epoch == 0) {
+      std::fill(stamps.begin(), stamps.end(), 0u);
+      epoch = 1;
+    }
+    return epoch;
   }
 };
 
@@ -90,18 +157,17 @@ struct Solver {
   unsigned char *tvirt;    // PodInfo.IsVirtualStatus
   // NodeInfo.PodInfos keeps a clone per node: a task evicted from A and pipelined to B sits on both (slots 0 and 1); a
   // victim that an earlier action moved and this one evicts and re-places sits on three or more: `on_extra` holds the
-  // (task, node, status) entries beyond the two slots (rare, linear look-up)
-  std::vector<int> &on_node0, &on_status0, &on_node1, &on_status1;
+  // (task, node, status) entries beyond the two slots (rare, linear look-up).  Slot 0 lives in the scratch (scr.n0 /
+  // scr.s0) for the tasks this action changed; for the others it is the snapshot's (node if active-used, node status).
+  SolverScratch &scr;
+  std::vector<int> &on_node1, &on_status1;
   std::vector<std::array<int, 3>> &on_extra;
   double *qa, *qnp;        // queue allocated / allocated-non-preemptible [3][Q]
   // GPU column of the host mirror of Idle / Releasing (seq.mirror, node-major; point look-ups only)
   double Ig(int n) const { return seq.mirror[(size_t)n * 2 * R + KAI_RES_GPU]; }
   double Lg(int n) const { return seq.mirror[(size_t)n * 2 * R + R + KAI_RES_GPU]; }
   // attempt-start values of touched rows (FeasibleNodesForJob and the filter's base map read the state the
-  // attempt started from)
-  std::vector<int> touched_epoch;
-  std::vector<double> startIg, startLg;
-  int epoch = 0;
+  // attempt started from): scr.start_ig / scr.start_lg, valid where scr.node_stamp equals scr.node_epoch
 
   enum { OPK_ALLOCATE = 0, OPK_PIPELINE = 1, OPK_EVICT = 2, OPK_UNDO = 3 };
   struct SOp {
@@ -114,18 +180,19 @@ struct Solver {
   long long n_vq_copy = 0, n_vq_build = 0;
   double t_sweeps = 0, t_sim_setup = 0, t_evict = 0, t_victims_queue = 0, t_vq_pop = 0, t_tte = 0, t_addp = 0, t_filter = 0, t_bypod = 0, t_finit = 0;
 
-  Solver(HostBackend &hb_, std::vector<int> &n0, std::vector<int> &s0, std::vector<int> &n1, std::vector<int> &s1,
+  Solver(HostBackend &hb_, SolverScratch &scratch, std::vector<int> &n1, std::vector<int> &s1,
          std::vector<std::array<int, 3>> &extra)
       : hb(hb_), seq(hb_.seq), ctl(hb_.ctl), s(*hb_.seq.s), cfg(*hb_.seq.cfg), N(s.N), Q(s.Q), J(s.J), S(s.S), T(s.T),
-        R(s.R), on_node0(n0), on_status0(s0), on_node1(n1), on_status1(s1), on_extra(extra) {
+        R(s.R), scr(scratch), on_node1(n1), on_status1(s1), on_extra(extra) {
     st = seq.rp.t_status;
     tn = seq.rp.t_node;
     tvirt = seq.rp.t_virtual;
     qa = seq.rp.q_alloc;
     qnp = seq.rp.q_alloc_np;
-    touched_epoch.assign(N, -1);
-    startIg.assign(N, 0);
-    startLg.assign(N, 0);
+    scr.size_for(N, J, T);
+    SolverScratch::bump(scr.slot_epoch, scr.slot_stamp);
+    scr.slot_list.clear();
+    setup_check = getenv("KAI_SOLVER_SETUP_CHECK") != nullptr;
     // Host answers need the mirror of every node and no topology term; with several GPUs every rank would answer alike,
     // but the multi-GPU path keeps its MINMAX exchange (DESIGN.md §7).
     const char *mx = getenv("KAI_HOST_SWEEP_MAX");
@@ -172,11 +239,7 @@ struct Solver {
   // ---------------- views: the session's jobs (id < J) and CloneWithTasks clones (job_info.go:477-510) ----------------
   // A clone owns copies of the PodSets: per-podset counters, Allocated and the inner caches are frozen at clone
   // time; the statuses of the tasks it lists stay live (the statement mutates the very PodInfo objects).
-  struct Cache {
-    bool tta_valid = false, res_valid = false;
-    std::vector<int> tta;
-    double res[QR] = {0, 0, 0};
-  };
+  typedef SolverJobCache Cache;
   struct View {
     int job = -1;
     std::vector<std::vector<int>> ps_tasks;
@@ -186,9 +249,16 @@ struct Solver {
     Cache cache;
   };
   std::vector<View> views;
-  std::vector<Cache> job_cache;  // live jobs: invalidated on every status change (job_info.go:281-284)
   int vjob(int v) const { return v < J ? v : views[v - J].job; }
-  Cache &vcache(int v) { return v < J ? job_cache[v] : views[v - J].cache; }
+  Cache &vcache(int v) {  // live jobs (scr.job_cache): invalidated per action and on every status change (job_info.go:281-284)
+    if (v >= J) return views[v - J].cache;
+    Cache &c = scr.job_cache[v];
+    if (c.stamp != scr.job_epoch) {
+      c.stamp = scr.job_epoch;
+      c.tta_valid = c.res_valid = false;
+    }
+    return c;
+  }
   int v_nps(int v) const { return ps_end(vjob(v)) - ps_begin(vjob(v)); }
   int v_min(int v, int k) const { return v < J ? s.ps_min[ps_begin(v) + k] : views[v - J].ps_min[k]; }
   int v_active_alloc(int v, int k) const {
@@ -325,16 +395,28 @@ struct Solver {
 
   // ---------------- node accounting: host mirror of the GPU column + deltas to the owning scanner ----------------
   void touch(int n) {
-    if (touched_epoch[n] != epoch) {
-      touched_epoch[n] = epoch;
-      startIg[n] = Ig(n);
-      startLg[n] = Lg(n);
+    if (scr.node_stamp[n] != scr.node_epoch) {
+      scr.node_stamp[n] = scr.node_epoch;
+      scr.start_ig[n] = Ig(n);
+      scr.start_lg[n] = Lg(n);
     }
   }
-  double start_Ig(int n) const { return touched_epoch[n] == epoch ? startIg[n] : Ig(n); }
-  double start_Lg(int n) const { return touched_epoch[n] == epoch ? startLg[n] : Lg(n); }
+  double start_Ig(int n) const { return scr.node_stamp[n] == scr.node_epoch ? scr.start_ig[n] : Ig(n); }
+  double start_Lg(int n) const { return scr.node_stamp[n] == scr.node_epoch ? scr.start_lg[n] : Lg(n); }
+  // slot 0 of task t: the snapshot's until the action first changes t (status, node or slots), then scr.n0 / scr.s0
+  int node0(int t) const {
+    if (scr.slot_stamp[t] == scr.slot_epoch) return scr.n0[t];
+    return (st[t] & kActiveUsed) && tn[t] >= 0 ? tn[t] : -1;
+  }
+  void take_slot(int t) {  // before the first change of t: copy its snapshot slot and list t for the teardown
+    if (scr.slot_stamp[t] == scr.slot_epoch) return;
+    scr.slot_stamp[t] = scr.slot_epoch;
+    scr.n0[t] = (st[t] & kActiveUsed) && tn[t] >= 0 ? tn[t] : -1;
+    scr.s0[t] = s.t_node_status[t];
+    scr.slot_list.push_back(t);
+  }
   int find_on(int t, int n) const {  // 0 / 1 = slot, 2 + i = on_extra[i], -1 = the task has no entry on node n
-    if (on_node0[t] == n) return 0;
+    if (node0(t) == n) return 0;
     if (on_node1[t] == n) return 1;
     for (size_t i = 0; i < on_extra.size(); i++)
       if (on_extra[i][0] == t && on_extra[i][1] == n) return 2 + (int)i;
@@ -366,27 +448,29 @@ struct Solver {
     }
   }
   void node_add_task(int t) {  // node_info.go:457-493 with the task's current status
+    take_slot(t);
     int n = tn[t], status = st[t];
     int e = find_on(t, n);
-    if (e < 0) e = on_node0[t] < 0 ? 0 : (on_node1[t] < 0 ? 1 : 2 + (int)on_extra.size());
+    if (e < 0) e = scr.n0[t] < 0 ? 0 : (on_node1[t] < 0 ? 1 : 2 + (int)on_extra.size());
     if (e >= 2) {
       if (e - 2 == (int)on_extra.size()) on_extra.push_back({t, n, status});
       on_extra[e - 2][2] = status;
     } else {
-      (e == 0 ? on_node0 : on_node1)[t] = n;
-      (e == 0 ? on_status0 : on_status1)[t] = status;
+      (e == 0 ? scr.n0 : on_node1)[t] = n;
+      (e == 0 ? scr.s0 : on_status1)[t] = status;
     }
     node_delta(t, n, status == KAI_POD_RELEASING ? ND_ADD_RELEASING : (status == KAI_POD_PIPELINED ? ND_ADD_PIPELINED : ND_ADD));
   }
   void node_remove_task(int t, int n) {  // :515-551 with the status of the clone stored on the node
+    take_slot(t);
     int e = find_on(t, n);
     if (e < 0) return;  // node_info.go:495-501: a pod that is no longer on the node is an error, the node is untouched
-    int status = e >= 2 ? on_extra[e - 2][2] : (e == 0 ? on_status0 : on_status1)[t];
+    int status = e >= 2 ? on_extra[e - 2][2] : (e == 0 ? scr.s0 : on_status1)[t];
     node_delta(t, n, status == KAI_POD_RELEASING ? ND_REM_RELEASING : (status == KAI_POD_PIPELINED ? ND_REM_PIPELINED : ND_REM));
     if (e >= 2)
       on_extra.erase(on_extra.begin() + (e - 2));
     else
-      (e == 0 ? on_node0 : on_node1)[t] = -1;
+      (e == 0 ? scr.n0 : on_node1)[t] = -1;
   }
   // jobs with Pending tasks (utils.GetAllPendingJobs, actions/utils/action.go:122-130), kept as statuses change
   std::vector<int> pending_cnt;
@@ -395,6 +479,7 @@ struct Solver {
   // victims queues ask it of every job of every leaf queue
   std::vector<int> ps_active;
   void set_status(int t, int status) {
+    take_slot(t);
     const int j = tjob(t);
     if (st[t] == KAI_POD_PENDING && status != KAI_POD_PENDING) {
       if (--pending_cnt[j] == 0) pending_jobs.erase(j);
@@ -404,7 +489,8 @@ struct Solver {
     const bool was_active = (st[t] & kActiveAllocated) != 0, is_active = (status & kActiveAllocated) != 0;
     if (was_active != is_active) ps_active[s.t_podset[t]] += is_active ? 1 : -1;
     st[t] = status;
-    job_cache[j].tta_valid = job_cache[j].res_valid = false;
+    Cache &c = vcache(j);
+    c.tta_valid = c.res_valid = false;
     if (s.j_queue[j] >= 0) leaf_epoch[s.j_queue[j]]++;
   }
   void queue_allocate(int t, bool add) {  // proportion.go:443-489
@@ -604,7 +690,7 @@ struct Solver {
   // instead of a GPU round trip.  No record is published: the queued node and feasible-set deltas stay queued for the
   // next record, so the scanners' tiles stay in step, and no sequence number is consumed.
   static constexpr int kHostSweepMaxDefault = 256;
-  static constexpr int kSeqErrHostSweep = 3;  // Seq::error: KAI_HOST_SWEEP_CHECK found a difference
+  static constexpr int kSeqErrHostSweep = 3;  // Seq::error: KAI_HOST_SWEEP_CHECK or KAI_SOLVER_SETUP_CHECK found a difference
   int host_sweep_max = 0;         // KAI_HOST_SWEEP_MAX (0: every sweep runs on the GPU)
   bool host_sweep_check = false;  // KAI_HOST_SWEEP_CHECK: run the GPU sweep as well and fail on any difference
   long long host_sweeps = 0;
@@ -888,21 +974,76 @@ struct Solver {
   }
 
   // ---------------- JobsOrderByQueues (actions/utils/job_order_by_queue.go) over views ----------------
+  // Flat form: every heap of the tree (root, queue nodes, leaves) is a range of one arena, nodes are plain data and the
+  // comparators are small function objects over the owning JobsOrder, so a copy is a few contiguous copies and a build
+  // allocates nothing per node.  A heap that outgrows its range moves to the end of the arena.
+  struct HeapRange {
+    int off = 0, len = 0, cap = 0;
+  };
   struct QNode {
     int queue = -1, parent = -1;
-    bool is_leaf = false, needs_reorder = false;
-    HeapGo<int> children;
+    bool is_leaf = false, needs_reorder = false, linked = false;
     int lazy_queue = -1;  // victims queue: only the best job of this leaf is loaded so far (Solver::victim_leaf_list has the rest)
+    HeapRange children;
+  };
+  struct JobsOrder;
+  struct JobLess {  // leaf heaps: JobOrderFn, inverted for the victims queue
+    const JobsOrder *jo;
+    bool operator()(int a, int b) const { return jo->victim_queue ? !jo->job_less(a, b) : jo->job_less(a, b); }
+  };
+  struct NodeLess {  // root and queue-node heaps: QueueOrderFn
+    JobsOrder *jo;
+    bool operator()(int a, int b) const { return jo->node_less(a, b); }
   };
   struct JobsOrder {
     Solver *o = nullptr;
     bool victim_queue = false;
     std::vector<QNode> nodes;
     std::vector<int> queue_node;
-    std::vector<char> linked;
-    HeapGo<int> root;
-    std::vector<std::vector<int>> popped_by_queue;
-    std::vector<double> popped_alloc;  // [Q][3] running Allocated sum of popped_by_queue (victims queue)
+    std::vector<int> arena;
+    HeapRange root;
+    std::vector<double> popped_alloc;  // [Q][3] running Allocated sum of the victims popped per queue (victims queue)
+
+    int *heap_data(const HeapRange &h) { return arena.data() + h.off; }
+    const int *heap_data(const HeapRange &h) const { return arena.data() + h.off; }
+    int peek(const HeapRange &h) const { return arena[h.off]; }
+    HeapRange &heap_of(int ni) { return ni < 0 ? root : nodes[ni].children; }  // ni = -1: the root heap
+    bool heap_is_leaf(int ni) const { return ni >= 0 && nodes[ni].is_leaf; }
+    void reserve_heap(int ni, int need) {  // room for `need` entries; moves the range to the end of the arena if short
+      HeapRange &h = heap_of(ni);
+      if (need <= h.cap) return;
+      const int cap = std::max(need, 2 * h.cap), off = (int)arena.size();
+      arena.resize((size_t)off + cap);
+      std::copy(arena.begin() + h.off, arena.begin() + h.off + h.len, arena.begin() + off);
+      h.off = off;
+      h.cap = cap;
+    }
+    void heap_assign(int ni, const int *src, int n) {  // the entries as they are (a sorted run is already a heap)
+      heap_of(ni).len = 0;
+      reserve_heap(ni, n);
+      HeapRange &h = heap_of(ni);
+      std::copy(src, src + n, arena.begin() + h.off);
+      h.len = n;
+    }
+    void heap_push(int ni, int x) {
+      reserve_heap(ni, heap_of(ni).len + 1);
+      HeapRange &h = heap_of(ni);
+      if (heap_is_leaf(ni))
+        HeapGo::push(heap_data(h), h.len, x, JobLess{this});
+      else
+        HeapGo::push(heap_data(h), h.len, x, NodeLess{this});
+    }
+    int heap_pop(int ni) {
+      HeapRange &h = heap_of(ni);
+      return heap_is_leaf(ni) ? HeapGo::pop(heap_data(h), h.len, JobLess{this}) : HeapGo::pop(heap_data(h), h.len, NodeLess{this});
+    }
+    void heap_fix(int ni, int i) {
+      HeapRange &h = heap_of(ni);
+      if (heap_is_leaf(ni))
+        HeapGo::fix(heap_data(h), h.len, i, JobLess{this});
+      else
+        HeapGo::fix(heap_data(h), h.len, i, NodeLess{this});
+    }
 
     void min_available_state(int v, bool &below, bool &above, bool &exactly) const {  // elastic.go:50-63
       exactly = true;
@@ -932,11 +1073,11 @@ struct Solver {
       if (la && re) return false;
       return o->s.j_order_rank[lj] < o->s.j_order_rank[rj];
     }
-    int best_job(int ni) const { return nodes[ni].is_leaf ? nodes[ni].children.peek() : best_job(nodes[ni].children.peek()); }
-    int leaf_of_best(int ni) const { return nodes[ni].is_leaf ? ni : leaf_of_best(nodes[ni].children.peek()); }
+    int best_job(int ni) const { return nodes[ni].is_leaf ? peek(nodes[ni].children) : best_job(peek(nodes[ni].children)); }
+    int leaf_of_best(int ni) const { return nodes[ni].is_leaf ? ni : leaf_of_best(peek(nodes[ni].children)); }
     bool node_less(int l, int r) {  // :256-278
-      if (nodes[l].children.empty()) return !victim_queue;
-      if (nodes[r].children.empty()) return victim_queue;
+      if (nodes[l].children.len == 0) return !victim_queue;
+      if (nodes[r].children.len == 0) return victim_queue;
       double lreq[QR] = {0, 0, 0}, rreq[QR] = {0, 0, 0}, lv[QR] = {0, 0, 0}, rv[QR] = {0, 0, 0};
       if (!victim_queue) {
         const double *a = o->tta_init_resource(best_job(l), false);
@@ -960,51 +1101,35 @@ struct Solver {
       int leaf = leaf_of_best(ni);
       const double *acc = popped_alloc.data() + (size_t)nodes[leaf].queue * QR;
       for (int r = 0; r < QR; r++) out[r] = acc[r];
-      if (!nodes[leaf].children.empty()) o->v_allocated(nodes[leaf].children.peek(), out);
-    }
-    // the comparators capture `this`: a copy must bind its own
-    void rebind() {
-      root.less = [this](const int &a, const int &b) { return node_less(a, b); };
-      for (auto &n : nodes) {
-        if (n.is_leaf)
-          n.children.less = [this](const int &a, const int &b) { return victim_queue ? !job_less(a, b) : job_less(a, b); };
-        else
-          n.children.less = [this](const int &a, const int &b) { return node_less(a, b); };
-      }
+      if (nodes[leaf].children.len != 0) o->v_allocated(peek(nodes[leaf].children), out);
     }
     void copy_from(const JobsOrder &src) {
       o = src.o;
       victim_queue = src.victim_queue;
       nodes = src.nodes;
       queue_node = src.queue_node;
-      linked = src.linked;
+      arena = src.arena;
       root = src.root;
-      popped_by_queue = src.popped_by_queue;
       popped_alloc = src.popped_alloc;
-      rebind();
     }
     void init(Solver *solver, bool victims) {
       o = solver;
       victim_queue = victims;
       nodes.clear();
-      nodes.reserve(4 * (size_t)o->Q + 16);
       queue_node.assign(o->Q, -1);
-      linked.clear();
-      popped_by_queue.assign(o->Q, {});
-      popped_alloc.assign((size_t)o->Q * QR, 0.0);
-      root = HeapGo<int>();
-      root.less = [this](const int &a, const int &b) { return node_less(a, b); };
+      arena.clear();
+      root = HeapRange();
+      if (victims)
+        popped_alloc.assign((size_t)o->Q * QR, 0.0);
+      else
+        popped_alloc.clear();
     }
-    int make_node(int q, bool leaf) {
+    int make_node(int q, bool leaf) {  // a queue node's heap holds at most its child queues
       nodes.emplace_back();
       int id = (int)nodes.size() - 1;
       nodes[id].queue = q;
       nodes[id].is_leaf = leaf;
-      if (leaf)
-        nodes[id].children.less = [this](const int &a, const int &b) { return victim_queue ? !job_less(a, b) : job_less(a, b); };
-      else
-        nodes[id].children.less = [this](const int &a, const int &b) { return node_less(a, b); };
-      linked.resize(nodes.size(), 0);
+      reserve_heap(id, leaf ? 1 : std::max(1, o->s.q_nchildren[q]));
       return id;
     }
     void mark_ancestors(int ni) {
@@ -1013,9 +1138,9 @@ struct Solver {
     void ensure_chain(int child) {  // :135-175
       int cq = nodes[child].queue;
       if (o->s.q_parent[cq] < 0) {
-        if (!linked[child]) {
-          root.push(child);
-          linked[child] = 1;
+        if (!nodes[child].linked) {
+          heap_push(-1, child);
+          nodes[child].linked = true;
         }
         return;
       }
@@ -1026,10 +1151,10 @@ struct Solver {
         pn = make_node(pq, false);
         queue_node[pq] = pn;
       }
-      if (!linked[child]) {
+      if (!nodes[child].linked) {
         nodes[child].parent = pn;
-        nodes[pn].children.push(child);
-        linked[child] = 1;
+        heap_push(pn, child);
+        nodes[child].linked = true;
       }
       if (is_new) ensure_chain(pn);
     }
@@ -1038,7 +1163,8 @@ struct Solver {
       if (nodes[leaf].lazy_queue < 0) return;
       const int q = nodes[leaf].lazy_queue;
       nodes[leaf].lazy_queue = -1;
-      nodes[leaf].children.a = o->victim_leaf_list(*this, q);  // same best job on top: the ancestors' heaps are unaffected
+      const std::vector<int> &run = o->victim_leaf_list(*this, q);  // same best job on top: the ancestors' heaps are unaffected
+      heap_assign(leaf, run.data(), (int)run.size());
     }
     void push_job(int v) {  // :90-119
       int q = o->s.j_queue[o->vjob(v)];
@@ -1050,32 +1176,30 @@ struct Solver {
         leaf = make_node(q, true);
         queue_node[q] = leaf;
       }
-      nodes[leaf].children.push(v);
+      heap_push(leaf, v);
       if (needs_linking) ensure_chain(leaf);
       mark_ancestors(leaf);
     }
-    bool is_empty() const { return root.empty(); }
-    int get_next_node(HeapGo<int> &pq) {  // :193-215
+    bool is_empty() const { return root.len == 0; }
+    int get_next_node(int hi) {  // :193-215 (hi: the heap's owner, -1 = root)
       for (;;) {
-        if (pq.empty()) return -1;
-        int ni = pq.peek();
+        const HeapRange &h = heap_of(hi);
+        if (h.len == 0) return -1;
+        int ni = peek(h);
         if (nodes[ni].needs_reorder) {
-          pq.fix(0);
+          heap_fix(hi, 0);
           nodes[ni].needs_reorder = false;
           continue;
         }
-        if (nodes[ni].children.empty()) return -1;
+        if (nodes[ni].children.len == 0) return -1;
         return ni;
       }
     }
     void handle_pop(int ni) {  // :219-243
-      if (nodes[ni].children.len() == 0) {
-        if (nodes[ni].parent >= 0)
-          nodes[nodes[ni].parent].children.pop();
-        else
-          root.pop();
+      if (nodes[ni].children.len == 0) {
+        heap_pop(nodes[ni].parent);  // parent -1: the root heap
         queue_node[nodes[ni].queue] = -1;
-        linked[ni] = 0;
+        nodes[ni].linked = false;
         if (nodes[ni].parent >= 0) handle_pop(nodes[ni].parent);
         return;
       }
@@ -1083,23 +1207,20 @@ struct Solver {
     }
     int pop_next_job() {  // :61-88
       if (is_empty()) return -1;
-      HeapGo<int> *pq = &root;
+      int hi = -1;
       int leaf = -1;
       for (;;) {
-        int ni = get_next_node(*pq);
+        int ni = get_next_node(hi);
         if (ni < 0) return -1;
         if (nodes[ni].is_leaf) {
           leaf = ni;
           break;
         }
-        pq = &nodes[ni].children;
+        hi = ni;
       }
       materialize(leaf);
-      int job = nodes[leaf].children.pop();
-      if (victim_queue) {
-        popped_by_queue[nodes[leaf].queue].push_back(job);
-        o->v_allocated(job, popped_alloc.data() + (size_t)nodes[leaf].queue * QR);
-      }
+      int job = heap_pop(leaf);
+      if (victim_queue) o->v_allocated(job, popped_alloc.data() + (size_t)nodes[leaf].queue * QR);
       handle_pop(leaf);
       return job;
     }
@@ -1173,7 +1294,6 @@ struct Solver {
     int k = 0;
     std::map<int, double> value;  // nodes of the base top-k and nodes that received victims' GPUs
     std::multiset<double, std::greater<double>> sorted;  // the same values, descending (incremental, like orderedInsert)
-    std::vector<char> seen;       // per task
     size_t n_rec_done = 0, n_pot_done = 0;
     std::vector<double> rq;  // GPU requests of the pending tasks, descending
   };
@@ -1182,8 +1302,8 @@ struct Solver {
     for (const std::vector<int> *lst : {&sc.recorded_tasks, &sc.potential_tasks})
       for (size_t i = (lst == &sc.recorded_tasks ? f.n_rec_done : f.n_pot_done); i < lst->size(); i++) {
         const int t = (*lst)[i];
-        if (tn[t] < 0 || f.seen[t]) continue;
-        f.seen[t] = 1;
+        if (tn[t] < 0 || scr.seen_stamp[t] == scr.seen_epoch) continue;
+        scr.seen_stamp[t] = scr.seen_epoch;
         auto it = f.value.find(tn[t]);
         if (it == f.value.end())
           it = f.value.emplace(tn[t], start_Ig(tn[t]) + start_Lg(tn[t])).first;
@@ -1197,7 +1317,7 @@ struct Solver {
   }
   void idle_filter_init(IdleFilter &f, const Scenario &sc, unsigned int snap_bits) {
     f.k = (int)sc.pending_tasks.size();
-    f.seen.assign(T, 0);
+    SolverScratch::bump(scr.seen_epoch, scr.seen_stamp);  // no task accounted yet
     for (auto &kv : sweep_topk_idle(f.k, snap_bits)) {
       f.value[kv.second] = kv.first;
       f.sorted.insert(kv.first);
@@ -1462,6 +1582,7 @@ struct Solver {
   }
 
   // ---------------- simulation (actions/common/action.go:67-122) ----------------
+  JobsOrder sim_order;  // the job order of the current simulation (kept for its capacity)
   bool try_virtually_allocate(const Scenario &sc, const std::vector<int> &victim_tasks) {
     const int pj = vjob(sc.preemptor);
     simulations++;
@@ -1474,7 +1595,7 @@ struct Solver {
     in_set.insert(pj);
     std::vector<int> vs;
     for (int j : in_set) vs.push_back(j == pj ? sc.preemptor : j);  // ascending job index, as before
-    JobsOrder jo;
+    JobsOrder &jo = sim_order;
     jo.init(this, false);
     init_jobs_order(jo, vs, OrderOpts());
     t_sim_setup += HostBackend::now() - t_setup0;
@@ -1673,7 +1794,7 @@ struct Solver {
         if (a.empty()) continue;
         const int leaf = jo.make_node(q, true);
         jo.queue_node[q] = leaf;
-        jo.nodes[leaf].children.a = a;
+        jo.heap_assign(leaf, a.data(), (int)a.size());
         jo.ensure_chain(leaf);
         jo.mark_ancestors(leaf);
         continue;
@@ -1683,7 +1804,7 @@ struct Solver {
       if (top < 0) continue;
       const int leaf = jo.make_node(q, true);
       jo.queue_node[q] = leaf;
-      jo.nodes[leaf].children.a.assign(1, top);
+      jo.heap_assign(leaf, &top, 1);
       jo.nodes[leaf].lazy_queue = q;
       jo.ensure_chain(leaf);
       jo.mark_ancestors(leaf);
@@ -1692,7 +1813,7 @@ struct Solver {
   }
   // the partial jobs of one pending job (job_solver.go:60-88) start from the same committed state: the queue built for
   // the first one is copied for the others (commit_epoch counts the statements committed in this action)
-  JobsOrder vq_proto;
+  JobsOrder vq_proto, vq_cur;  // vq_cur: the victims queue of the partial job being solved (kept for its capacity)
   int vq_proto_job = -1, vq_proto_kind = -1;
   long long vq_proto_commit = -1, commit_epoch = 0;
   void build_victims_queue(JobsOrder &jo, int pending_job) {
@@ -1758,9 +1879,9 @@ struct Solver {
     for (int rv : state.recorded_jobs) scenario_append_group(sc, v_all_tasks(rv));
     for (int rv : state.recorded_jobs)
       for (int t : v_all_tasks(rv)) sc.recorded_tasks.push_back(t);
-    std::vector<char> recorded_set(T, 0);
-    for (int t : sc.recorded_tasks) recorded_set[t] = 1;
-    JobsOrder victims_queue;
+    const unsigned rec = SolverScratch::bump(scr.rec_epoch, scr.rec_stamp);
+    for (int t : sc.recorded_tasks) scr.rec_stamp[t] = rec;
+    JobsOrder &victims_queue = vq_cur;
     {
       const double t0 = HostBackend::now();
       build_victims_queue(victims_queue, pending_job);
@@ -1790,11 +1911,11 @@ struct Solver {
             t_tte += HostBackend::now() - tq;
             bool hit = false;
             for (int t : tasks)
-              if (recorded_set[t]) hit = true;
+              if (scr.rec_stamp[t] == rec) hit = true;
             if (hit) {
               std::vector<int> remaining;
               for (int t : v_all_tasks(next))
-                if (!recorded_set[t]) remaining.push_back(t);
+                if (scr.rec_stamp[t] != rec) remaining.push_back(t);
               if (!remaining.empty()) victims_queue.push_job(make_clone(next, remaining));
               continue;
             }
@@ -1865,9 +1986,9 @@ struct Solver {
   }
   // starts a job attempt: the next TOPK record snapshots FeasibleNodesForJob (feasible_nodes.go:11-26)
   void begin_attempt(int j) {
-    epoch++;
+    SolverScratch::bump(scr.node_epoch, scr.node_stamp);
+    for (int n : feas_extra_list) feas_extra[n] = 0;  // feas_extra is set exactly on feas_extra_list
     feas_extra_list.clear();
-    std::fill(feas_extra.begin(), feas_extra.end(), 0);
     feas_all = false;
     for (int ps = ps_begin(j); ps < ps_end(j); ps++)
       for (int t = pst_begin(ps); t < pst_end(ps); t++)
@@ -1929,23 +2050,52 @@ struct Solver {
     m[job_signature[j]] = j;
   }
 
+  // KAI_SOLVER_SETUP_CHECK (tests): recount what prepare() took from the prepare kernels by scanning every task status,
+  // and fail the action on any difference
+  bool setup_check = false;
+  void setup_fail(const char *field, int index, long long got, long long want) {
+    snprintf(hb.error_msg, sizeof(hb.error_msg), "KAI_SOLVER_SETUP_CHECK: %s[%d] is %lld, a recount of the task statuses gives %lld",
+             field, index, got, want);
+    seq.error = kSeqErrHostSweep;
+  }
+  void check_setup_counts() {
+    std::vector<int> act(S, 0), pend(J, 0);
+    for (int t = 0; t < T; t++) {
+      if (st[t] == KAI_POD_PENDING) pend[tjob(t)]++;
+      if (st[t] & kActiveAllocated) act[s.t_podset[t]]++;
+    }
+    for (int ps = 0; ps < S; ps++)
+      if (ps_active[ps] != act[ps]) return setup_fail("ps_active", ps, ps_active[ps], act[ps]);
+    for (int j = 0; j < J; j++) {
+      if (pending_cnt[j] != pend[j]) return setup_fail("pending_cnt", j, pending_cnt[j], pend[j]);
+      if ((pending_jobs.count(j) != 0) != (pend[j] > 0)) return setup_fail("pending_jobs", j, (long long)pending_jobs.count(j), pend[j] > 0);
+    }
+  }
+
   double t_prepare = 0;
   void prepare() {
     const double t0 = HostBackend::now();
-    job_cache.assign(J, Cache());
+    SolverScratch::bump(scr.job_epoch, scr.job_cache, &Cache::stamp);  // every job cache of an earlier action is stale
+    SolverScratch::bump(scr.node_epoch, scr.node_stamp);
     vq_leaf.assign(Q, {});
     vq_leaf_epoch.assign(Q, -1);
     vq_top.assign(Q, -1);
     vq_top_epoch.assign(Q, -1);
     leaf_epoch.assign(Q, 0);
+    // per-podset active-allocated and pending counts from k_prep_jobs (ps_cnt0, same masks, over the statuses this
+    // action starts from: nothing changes a status between that kernel's copy-back and here)
+    ps_active.assign(s.ps_cnt0, s.ps_cnt0 + S);
     pending_cnt.assign(J, 0);
     pending_jobs.clear();
-    ps_active.assign(S, 0);
-    for (int t = 0; t < T; t++) {
-      if (st[t] == KAI_POD_PENDING && pending_cnt[tjob(t)]++ == 0) pending_jobs.insert(tjob(t));
-      if (st[t] & kActiveAllocated) ps_active[s.t_podset[t]]++;
+    for (int j = 0; j < J; j++) {
+      int c = 0;
+      for (int ps = ps_begin(j); ps < ps_end(j); ps++) c += s.ps_cnt0[S + ps];
+      pending_cnt[j] = c;
+      if (c > 0) pending_jobs.insert(pending_jobs.end(), j);
     }
+    if (setup_check) check_setup_counts();
     feas_extra.assign(N, 0);
+    feas_extra_list.clear();
     ops_truncate(0);
     free_ready = 0;  // once per action, from the mirror of the GPU column the action starts with
     base_known = false;
