@@ -307,8 +307,8 @@ int kai_engine_load_snapshot(kai_engine *e, const kai_snapshot *snap);
    actions/reclaim/reclaim.go:46-119, actions/preempt/preempt.go:46-123,
    actions/stalegangeviction/stalegangeviction.go:29-95).  Session state persists between calls so that
    `allocate, consolidation, reclaim, preempt, stalegangeviction` run in sequence on one loaded snapshot.
-   Errors: KAI_ERR_UNSUPPORTED for combinations the engine does not run (victim-selection actions or topology
-   constraints with KAI_SEQUENCER=device); the session is then unchanged and the caller runs the stock action. */
+   Errors: KAI_ERR_UNSUPPORTED for inputs the engine does not run (KAI_TRANSPORT=persistent or KAI_SEQUENCER=device
+   in the environment: modes it no longer has); the session is then unchanged and the caller runs the stock action. */
 int kai_engine_run(kai_engine *e, kai_action action, kai_result *out);
 
 /* replaces: fairshare-simulator's SetResourcesShare call

@@ -3,17 +3,12 @@
 //   k_prep_jobs      per job: podset status counters, readiness, JobOrderFn sort key, cached
 //                    GetTasksToAllocateInitResource, "fresh uniform gang" flag                (grid-parallel)
 //   k_prep_queues    per leaf queue: eligible jobs in JobOrderFn order                        (CTA per queue)
-//   k_record         launch transport (default): ONE decision record per launch, 256 scanners x 128 threads.  Every
-//                    scanner owns a stripe of node rows (tile, resident in global memory / L2 between launches, staged
-//                    in shared memory for the sweep), applies the node deltas addressed to it, evaluates fit + score of
+//   k_record         ONE decision record of the host sequencer per launch, 256 scanners x 128 threads.  Every scanner
+//                    owns a stripe of node rows (tile, resident in global memory / L2 between launches, staged in
+//                    shared memory for the sweep), applies the node deltas addressed to it, evaluates fit + score of
 //                    its rows and answers: top-M candidates (lists), or one slot reduced by the last CTA to finish.
-//   k_merge_cluster  (k_merge: one-CTA form) sorts the scanners' candidates, cuts the list where an unseen row could be
-//                    better and streams it to host memory — the next launch on the stream after a list sweep.
-//   k_action         the same scanner code as ONE persistent cooperative kernel (one CTA per SM, tiles in shared memory
-//                    for the whole action): CTA 0 relays the records the host writes into pinned mapped memory
-//                    (KAI_TRANSPORT=persistent) or runs the sequencer itself (KAI_SEQUENCER=device): a 16-word decision
-//                    record (tagged 128-bit relaxed stores) plus the node deltas since the previous record go out,
-//                    one slot / M list lines per scanner come back.
+//   k_merge_cluster  sorts the scanners' candidates, cuts the list where an unseen row could be better and streams it
+//                    to host memory — the next launch on the stream after a list sweep.
 //
 // Exactness notes
 //   * FittingNode + NodeOrderFn + sortNodesByScore (framework/session.go:201-264,466-485) are evaluated as
@@ -405,8 +400,7 @@ constexpr int kSlotWords = 8;
 // (i = 0 is the swept placement, i >= 1 are candidate repeats on the same node); lane 0 then walks the
 // placements in order to simulate the min/max trackers and decides how many repeats it can vouch for.
 __device__ void publish_candidate(const Track *trk, const Tile &tl, const Decision &d, Cand local,
-                                  unsigned long long *slot, unsigned int tag, int batching, bool sys,
-                                  long long *dbg = nullptr) {
+                                  unsigned long long *slot, unsigned int tag, int batching, long long *dbg = nullptr) {
   const int lane = threadIdx.x & 31;
   long long d0 = clock64(), d1 = d0, d2 = d0, d3 = d0;
   local.score = __shfl_sync(0xffffffffu, local.score, 0);
@@ -562,23 +556,17 @@ __device__ void publish_candidate(const Track *trk, const Tile &tl, const Decisi
     dbg[1] += d2 - d1;
     dbg[2] += d3 - d2;
   }
-  auto put = [&](unsigned long long *w, unsigned long long lo, unsigned long long hi2) {
-    if (sys)
-      st_relaxed_sys_b128(w, lo, hi2);  // slot lives in pinned host memory (host-sequenced mode)
-    else
-      st_relaxed_b128(w, lo, hi2);
-  };
-  put(slot + 2, (unsigned long long)__double_as_longlong(a_gpu), (unsigned long long)tag);
-  put(slot + 4, (unsigned long long)__double_as_longlong(a_cpu), (unsigned long long)tag);
-  if (repeat) put(slot + 6, rep_flags, (unsigned long long)tag);
+  st_relaxed_b128(slot + 2, (unsigned long long)__double_as_longlong(a_gpu), (unsigned long long)tag);
+  st_relaxed_b128(slot + 4, (unsigned long long)__double_as_longlong(a_cpu), (unsigned long long)tag);
+  if (repeat) st_relaxed_b128(slot + 6, rep_flags, (unsigned long long)tag);
   unsigned long long hi = ((unsigned long long)tag << 40) | ((unsigned long long)(flags & 0xffu) << 32) |
                           ((unsigned long long)(repeat & 0xffu) << 24) | (unsigned long long)(local.rank & 0xffffffu);
-  put(slot, (unsigned long long)__double_as_longlong(local.score), hi);
+  st_relaxed_b128(slot, (unsigned long long)__double_as_longlong(local.score), hi);
 }
 
 
 // ---------------------------------------------------------------------------------------------
-// top-M answer (host-sequenced mode).  Warp w analyses candidate w: how many further identical pods the row can
+// top-M answer.  Warp w analyses candidate w: how many further identical pods the row can
 // take while staying at or above its own winning score in the same mode (repeat), and whether it is exhausted
 // afterwards (does not fit any more).  The host merges the lists of all scanners, simulates the min/max trackers
 // itself from the row values (same f64 operations) and consumes the list in key order (DESIGN.md §5).
@@ -680,7 +668,7 @@ __device__ void publish_list_candidate(const Tile &tl, const Decision &d, Cand c
 }
 
 // =============================================================================================
-// sequencer <-> scanner protocol
+// device-side exchanges inside one launch
 // =============================================================================================
 // Watchdog for the spin waits: a wait that does not complete within ~2^22 polls records (code, seq, who)
 // in counters[24..27], raises the abort flag and lets every waiter fall through so that the kernel ends
@@ -702,220 +690,13 @@ struct Spin {
     return false;
   }
 };
-// Publish the next decision record (warp 0 of CTA 0; lane 0 has prepared ctl.dec / trackers / deltas).
-__device__ void seq_publish(const ActionParams &p, Ctl &ctl, int kind) {
-  const int lane = threadIdx.x & 31;
-  if (lane == 0) {
-    close_delta(ctl, p.delta);
-    build_decision_words(ctl, kind, p.batching);  // deltas are self-validating tagged words: no fence
-  }
-  __syncwarp();
-  unsigned long long *rec = p.dbuf + (size_t)(ctl.seq & 1) * kDecWords * 2;
-  if (lane < kDecWords) st_relaxed_b128(rec + 2 * lane, ctl.dw[lane], (unsigned long long)ctl.seq);
-  __syncwarp();
-}
 
-// Gather the candidate slots of all scanners (warp 0 of CTA 0) and let lane 0 digest the winner.
-__device__ void seq_gather_candidates(const ActionParams &p, Ctl &ctl) {
-  const int lane = threadIdx.x & 31;
-  const unsigned int seq = ctl.seq;
-  unsigned long long *buf = p.xbuf + (size_t)(seq & 1) * kMaxGrid * kSlotWords;
-  const unsigned int tag = seq & 0xffffffu;
-  double bs = -1.0;
-  uint32_t brank = kRankNone, bmeta = 0;
-  int bslot = -1;
-  for (int c = lane; c < p.grid - 1; c += 32) {
-    const unsigned long long *slot = buf + (size_t)c * kSlotWords;
-    unsigned long long lo, hi;
-    {
-      Spin spin;
-      do {
-        ld_relaxed_b128(slot, lo, hi);
-      } while (((unsigned int)(hi >> 40) != tag) && !spin.expired(p, 1, (unsigned int)seq, (int)(c)));
-    }
-    double sc = __longlong_as_double((long long)lo);
-    uint32_t rk = (uint32_t)(hi & 0xffffffu);
-    if (better(sc, rk, bs, brank)) {
-      bs = sc;
-      brank = rk;
-      bmeta = (uint32_t)((hi >> 24) & 0xffffu);  // [flags:8][repeat:8]
-      bslot = c;
-    }
-  }
-  for (int o = 16; o > 0; o >>= 1) {
-    double os = __shfl_xor_sync(0xffffffffu, bs, o);
-    uint32_t orank = __shfl_xor_sync(0xffffffffu, brank, o);
-    uint32_t om = __shfl_xor_sync(0xffffffffu, bmeta, o);
-    int osl = __shfl_xor_sync(0xffffffffu, bslot, o);
-    if (better(os, orank, bs, brank)) {
-      bs = os;
-      brank = orank;
-      bmeta = om;
-      bslot = osl;
-    }
-  }
-  if (lane == 0) {
-    uint32_t bflags = bmeta >> 8, repeat = bmeta & 0xffu;
-    ctl.win.score = bs;
-    ctl.win.rank = brank;
-    ctl.win.flags = bflags;
-    ctl.win.node = brank == kRankNone ? -1 : __ldg(&p.s.rank_to_node[brank]);
-    ctl.batch.valid = 0;
-    if (brank != kRankNone) {
-      const unsigned long long *slot = buf + (size_t)bslot * kSlotWords;
-      for (int k = 0; k < 2; k++) {
-        uint32_t f = (bflags >> (3 * k)) & 7u;
-        double a = 0;
-        if (f & WF_A_LT_MN) {  // a new global minimum: fetch its value
-          unsigned long long lo, hi;
-          {
-            Spin spin;
-            do {
-              ld_relaxed_b128(slot + 2 + 2 * k, lo, hi);
-            } while (((unsigned int)hi != tag) && !spin.expired(p, 2, (unsigned int)seq, (int)(bslot)));
-          }
-          a = __longlong_as_double((long long)lo);
-        }
-        if (f) track_decrease(ctl.trk[k], f, a);
-      }
-      if (repeat) {
-        unsigned long long lo, hi;
-        {
-          Spin spin;
-          do {
-            ld_relaxed_b128(slot + 6, lo, hi);
-          } while (((unsigned int)hi != tag) && !spin.expired(p, 3, (unsigned int)seq, (int)(bslot)));
-        }
-        ctl.batch.valid = 1;
-        ctl.batch.node = ctl.win.node;
-        ctl.batch.to_idle = (bflags & SLOT_TO_IDLE) ? 1 : 0;
-        ctl.batch.left = (int)repeat;
-        ctl.batch.idx = 0;
-        ctl.batch.fl = lo;
-      }
-    }
-    ctl.seq = seq + 1;
-    ctl.n_delta = 0;
-  }
-  __syncwarp();
-}
-
-// min/max answer slots: four tagged words {value, [tag:32][count:32]} = gpu mn, gpu mx, cpu mn, cpu mx
-__device__ void seq_gather_minmax(const ActionParams &p, Ctl &ctl) {
-  const int lane = threadIdx.x & 31;
-  const unsigned int seq = ctl.seq;
-  unsigned long long *buf = p.mmbuf + (size_t)(seq & 1) * kMaxGrid * kSlotWords;
-  const unsigned long long tag = seq;
-  double gmn[2] = {DBL_MAX, DBL_MAX}, gmx[2] = {0, 0};
-  long long cmn[2] = {0, 0}, cmx[2] = {0, 0};
-  for (int cta = lane; cta < p.grid - 1; cta += 32) {
-    const unsigned long long *slot = buf + (size_t)cta * kSlotWords;
-    for (int k = 0; k < 2; k++) {
-      unsigned long long lo, hi;
-      {
-        Spin spin;
-        do {
-          ld_relaxed_b128(slot + 4 * k, lo, hi);
-        } while (((hi >> 32) != (tag & 0xffffffffu)) && !spin.expired(p, 4, (unsigned int)seq, (int)(cta)));
-      }
-      double v = __longlong_as_double((long long)lo);
-      int cnt = (int)(hi & 0xffffffffu);
-      if (cnt > 0) {
-        if (cmn[k] == 0 || v < gmn[k]) {
-          gmn[k] = v;
-          cmn[k] = cnt;
-        } else if (v == gmn[k])
-          cmn[k] += cnt;
-      }
-      {
-        Spin spin;
-        do {
-          ld_relaxed_b128(slot + 4 * k + 2, lo, hi);
-        } while (((hi >> 32) != (tag & 0xffffffffu)) && !spin.expired(p, 5, (unsigned int)seq, (int)(cta)));
-      }
-      v = __longlong_as_double((long long)lo);
-      cnt = (int)(hi & 0xffffffffu);
-      if (cnt > 0) {
-        if (cmx[k] == 0 || v > gmx[k]) {
-          gmx[k] = v;
-          cmx[k] = cnt;
-        } else if (v == gmx[k])
-          cmx[k] += cnt;
-      }
-    }
-  }
-  for (int k = 0; k < 2; k++)
-    for (int o = 16; o > 0; o >>= 1) {
-      double omn = __shfl_xor_sync(0xffffffffu, gmn[k], o);
-      long long ocmn = __shfl_xor_sync(0xffffffffu, cmn[k], o);
-      double omx = __shfl_xor_sync(0xffffffffu, gmx[k], o);
-      long long ocmx = __shfl_xor_sync(0xffffffffu, cmx[k], o);
-      if (ocmn > 0) {
-        if (cmn[k] == 0 || omn < gmn[k]) {
-          gmn[k] = omn;
-          cmn[k] = ocmn;
-        } else if (omn == gmn[k])
-          cmn[k] += ocmn;
-      }
-      if (ocmx > 0) {
-        if (cmx[k] == 0 || omx > gmx[k]) {
-          gmx[k] = omx;
-          cmx[k] = ocmx;
-        } else if (omx == gmx[k])
-          cmx[k] += ocmx;
-      }
-    }
-  if (lane == 0) {
-    for (int k = 0; k < 2; k++) {  // pack.go:66-86: min starts at MaxFloat64, max at 0
-      ctl.trk[k].mn = cmn[k] > 0 ? gmn[k] : DBL_MAX;
-      ctl.trk[k].mx = (cmx[k] > 0 && gmx[k] > 0) ? gmx[k] : 0.0;
-      ctl.trk[k].cnt_mn = (int)cmn[k];
-      ctl.trk[k].cnt_mx = (int)cmx[k];
-      ctl.trk[k].dirty = 0;
-    }
-    ctl.seq = seq + 1;
-    ctl.n_delta = 0;
-  }
-  __syncwarp();
-}
-
-// FLUSH issued by lane 0 alone from inside sequential code (delta list full; rare)
-__device__ void dev_flush_deltas(Seq &q) {
-  const ActionParams &p = *q.p;
-  Ctl &c = *q.ctl;
-  close_delta(c, q.delta_base);
-  build_decision_words(c, DK_FLUSH, 0);
-  unsigned long long *rec = p.dbuf + (size_t)(c.seq & 1) * kDecWords * 2;
-  for (int i = 0; i < kDecWords; i++) st_relaxed_b128(rec + 2 * i, c.dw[i], (unsigned long long)c.seq);
-  unsigned long long *buf = p.xbuf + (size_t)(c.seq & 1) * kMaxGrid * kSlotWords;
-  const unsigned int tag = c.seq & 0xffffffu;
-  for (int cta = 0; cta < p.grid - 1; cta++) {
-    unsigned long long lo, hi;
-    {
-      Spin spin;
-      do {
-        ld_relaxed_b128(buf + (size_t)cta * kSlotWords, lo, hi);
-      } while (((unsigned int)(hi >> 40) != tag) && !spin.expired(p, 6, (unsigned int)c.seq, (int)(cta)));
-    }
-  }
-  c.seq++;
-  c.n_delta = 0;
-}
-
-void host_flush_deltas(Seq &q);  // kai_host_seq.cuh
-KAI_HD void seq_flush_deltas(Seq &q) {
-#ifdef __CUDA_ARCH__
-  dev_flush_deltas(q);
-#else
-  host_flush_deltas(q);
-#endif
-}
 
 // =============================================================================================
 // scanner CTA
 // =============================================================================================
-// the arrays of a tile inside one contiguous block (shared memory of a persistent scanner, or the scanner's block of
-// g_tiles; the launch transport copies the latter into shared memory for the sweep, same offsets)
+// the arrays of a tile inside one contiguous block (the scanner's block of g_tiles, or its copy in shared memory that a
+// sweep reads; same offsets)
 __device__ __forceinline__ void tile_carve(Tile &tile, unsigned char *ptr) {
   const int npc = tile.npc;
   tile.I = (double *)ptr;
@@ -947,30 +728,30 @@ struct ScanShared {
   int2 delta[kMaxDelta];
   unsigned int mine_bits[kMaxDelta / 32], ext_bits[kMaxDelta / 32];  // per 32 list entries: owned by this scanner / extended
   int fit_count;
-  int ext_dirty;  // launch transport: the preferred-level score table changed in this launch
+  int ext_dirty;  // the preferred-level score table changed in this launch
   int excl[kTopM];
   Cand cands[kTopM];
   double dreq[kMaxDelta][KAI_MAX_RES];
   int dln[kMaxDelta];
 };
 
-// LAUNCH = false: persistent scanner (tile in shared memory, records polled from the device-side record buffer until DONE).
-// LAUNCH = true:  one launch = one record (`lrec`, kernel parameter); the tile lives in global memory between launches
-//                 (same layout), DK_LOAD fills it from the session tables, DK_DONE writes it back.  Returns true when
-//                 the record asks for an answer (the caller then runs the last-CTA reduction).
-template <bool LAUNCH>
+
+// One launch = one decision record (`lrec`, kernel parameter).  The tile lives in global memory between launches, in
+// the layout tile_carve() gives it; DK_LOAD fills it from the session tables, DK_DONE writes it back.  Returns true
+// when the record asks for an answer (the caller then runs the last-CTA reduction).
 __device__ bool scanner_main(const ActionParams &p, const LaunchRec *lrec, unsigned char *smem, Cand *sh_warp, double *sh_d,
                              int *sh_i, ScanShared &sh, Tile &tile) {
   const DevSnap &s = p.s;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nw = blockDim.x >> 5;
-  const int my = LAUNCH ? (int)blockIdx.x : (int)blockIdx.x - 1;
-  unsigned char *gstate = LAUNCH ? p.g_scan_state + (size_t)my * kScanStateBytes : nullptr;
+  const int my = (int)blockIdx.x;
+  unsigned char *gstate = p.g_scan_state + (size_t)my * kScanStateBytes;
+  const bool load_tile = (int)(lrec->dw[0] & 0xff) == DK_LOAD;
   if (tid == 0) {
     int npc = p.nodes_per_cta;
-    unsigned char *ptr = LAUNCH ? p.g_tiles + (size_t)my * p.g_tile_stride : smem;
+    unsigned char *ptr = p.g_tiles + (size_t)my * p.g_tile_stride;
     tile.npc = npc;
     tile.R = s.R;
-    tile.nscan = p.grid - 1;
+    tile.nscan = p.scanners;
     tile.nscan_log2 = (tile.nscan > 0 && (tile.nscan & (tile.nscan - 1)) == 0) ? 31 - __clz(tile.nscan) : -1;
     tile.my = my;
     tile.nshard = p.cfg.shard_count;
@@ -983,208 +764,171 @@ __device__ bool scanner_main(const ActionParams &p, const LaunchRec *lrec, unsig
     tile_carve(tile, ptr);
     sh.pref_level = -1;
     sh.ext_dirty = 0;
-    if (LAUNCH && (int)(lrec->dw[0] & 0xff) != DK_LOAD) sh.pref_level = *(const int *)gstate;
+    if (!load_tile) sh.pref_level = *(const int *)gstate;
   }
   __syncthreads();
-  const bool load_tile = !LAUNCH || (int)(lrec->dw[0] & 0xff) == DK_LOAD;
-  if (LAUNCH && !load_tile && sh.pref_level >= 0)  // the score buckets of the preferred level persist between launches
+  if (!load_tile && sh.pref_level >= 0)  // the score buckets of the preferred level persist between launches
     for (int i = tid; i < kDomBuckets; i += blockDim.x) sh.dom_bucket[i] = gstate[16 + i];
-  for (int ln = tid; load_tile && ln < tile.count; ln += blockDim.x) {
-    const int rk = tile_row_rank(tile, ln);
-    const int n = s.rank_to_node[rk];
-    tile.node[ln] = n;
-    for (int r = 0; r < s.R; r++) {
-      tile.I[r * tile.npc + ln] = s.idle[(size_t)r * s.N + n];
-      tile.L[r * tile.npc + ln] = s.rel[(size_t)r * s.N + n];
+  if (load_tile) {
+    for (int ln = tid; ln < tile.count; ln += blockDim.x) {
+      const int rk = tile_row_rank(tile, ln);
+      const int n = s.rank_to_node[rk];
+      tile.node[ln] = n;
+      for (int r = 0; r < s.R; r++) {
+        tile.I[r * tile.npc + ln] = s.idle[(size_t)r * s.N + n];
+        tile.L[r * tile.npc + ln] = s.rel[(size_t)r * s.N + n];
+      }
+      tile.Agpu[ln] = s.alloc[(size_t)KAI_RES_GPU * s.N + n];
+      tile.Acpu[ln] = s.alloc[(size_t)KAI_RES_CPU * s.N + n];
+      tile.gpu_count[ln] = s.gpu_count[n];
+      tile.rank[ln] = rk;
+      tile.flags[ln] = s.nflags[n];
+      for (int l = 0; l < tile.n_dom_levels; l++) tile.dom[l * tile.npc + ln] = p.node_domain[(size_t)l * s.N + n];
     }
-    tile.Agpu[ln] = s.alloc[(size_t)KAI_RES_GPU * s.N + n];
-    tile.Acpu[ln] = s.alloc[(size_t)KAI_RES_CPU * s.N + n];
-    tile.gpu_count[ln] = s.gpu_count[n];
-    tile.rank[ln] = rk;
-    tile.flags[ln] = s.nflags[n];
-    for (int l = 0; l < tile.n_dom_levels; l++) tile.dom[l * tile.npc + ln] = p.node_domain[(size_t)l * s.N + n];
-  }
-  __syncthreads();
-  if (LAUNCH && load_tile) {
+    __syncthreads();
     if (tid == 0) *(int *)gstate = -1;
     return false;
   }
-  unsigned int seq = LAUNCH ? lrec->seq : p.seq0;
+  const unsigned int seq = lrec->seq;
   long long ts[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-  bool wrote_answer = false;
-  for (;;) {
-    long long c0 = clock64();
-    // ---- wait for decision record `seq` ----
-    if (LAUNCH) {
-      if (tid < kDecWords) sh.dw[tid] = lrec->dw[tid];
-    } else if (warp == 0) {
-      const unsigned long long *rec0 = p.dbuf + (size_t)(seq & 1) * kDecWords * 2;
-      if (lane == 0) {  // one poller per CTA on word 0 keeps the record's L2 lines cool
-        unsigned long long lo, hi;
-        Spin spin;
-        for (;;) {
-          ld_relaxed_b128(rec0, lo, hi);
-          if (hi == (unsigned long long)seq || spin.expired(p, 7, seq, 0)) break;
-          __nanosleep(20);
-        }
+  long long c0 = clock64();
+  if (tid < kDecWords) sh.dw[tid] = lrec->dw[tid];
+  __syncthreads();
+  long long c1 = clock64();
+  if (tid < 32) {  // decode in parallel: lane r writes req[r], lanes 8/9 the trackers, lane 10 the scalars
+    const unsigned long long w0 = sh.dw[0];
+    const unsigned int bits = (unsigned int)((w0 >> 24) & 0xff);
+    Decision &d = sh.dec;
+    if (tid < KAI_MAX_RES) d.req[tid] = __longlong_as_double((long long)sh.dw[2 + tid]);
+    if (tid == 8 || tid == 9) {
+      const int k = tid - 8;
+      sh.trk[k].mn = __longlong_as_double((long long)sh.dw[10 + 2 * k]);
+      sh.trk[k].mx = __longlong_as_double((long long)sh.dw[11 + 2 * k]);
+      sh.trk[k].cnt_mn = (int)(unsigned int)(sh.dw[14 + k] & 0xffffffffu);
+      sh.trk[k].cnt_mx = (int)(unsigned int)(sh.dw[14 + k] >> 32);
+      sh.trk[k].dirty = (bits & (k == 0 ? DB_DIRTY0 : DB_DIRTY1)) ? 1 : 0;
+    }
+    if (tid == 10) {
+      sh.kind = (int)(w0 & 0xff);
+      d.res = (int)((w0 >> 8) & 0xff);
+      d.strategy = (int)((w0 >> 16) & 0xff);
+      sh.n_delta = (int)((w0 >> 32) & 0xffff);
+      sh.xbits = (int)((w0 >> 48) & 0xffff);
+      d.restricted = (sh.xbits & XB_RESTRICT) ? 1 : 0;
+      d.gpu_task = (bits & DB_GPU_TASK) ? 1 : 0;
+      d.best_effort = (bits & DB_BEST_EFFORT) ? 1 : 0;
+      d.pipeline_only = (bits & DB_PIPELINE_ONLY) ? 1 : 0;
+      sh.batching = (bits & DB_BATCHING) ? 1 : 0;
+      d.nominated = (int)(unsigned int)(sh.dw[1] & 0xffffffffu);
+      d.pred_class = (int)(unsigned int)(sh.dw[1] >> 32);
+      const int tk = d.res == KAI_RES_GPU ? 0 : 1;
+      d.mn = __longlong_as_double((long long)sh.dw[10 + 2 * tk]);
+      d.mx = __longlong_as_double((long long)sh.dw[11 + 2 * tk]);
+      d.task = -1;
+    }
+  }
+  __syncthreads();
+  long long c2 = clock64();
+  // ---- apply the node deltas that belong to this tile (loads in parallel, application in list order) ----
+  // Every scanner sees the whole list but owns ~1/scanners of it: the entries are classified in parallel (ballot bits
+  // per 32 entries: "mine", "extended") and only the set bits are walked, in list order.
+  const int nd = sh.n_delta;
+  if (nd > 0) {
+    for (int e0 = 0; e0 < nd; e0 += blockDim.x) {
+      const int e = e0 + tid;
+      bool mine = false, ext = false;
+      if (e < nd) {
+        const unsigned long long lo = (unsigned long long)lrec->dkey[e] | ((unsigned long long)lrec->dtask[e] << 32);
+        const unsigned long long hi = (unsigned long long)seq | ((unsigned long long)lrec->dcount[e] << 32);
+        int2 en = make_int2((int)(unsigned int)(lo & 0xffffffffu), (int)(unsigned int)(lo >> 32));
+        sh.delta[e] = en;
+        int ln = 0;
+        ext = en.x < 0;
+        mine = en.x >= 0 && tile_owns(tile, (unsigned int)(en.x & 0x0fffffff), ln) && ln < tile.count;
+        sh.dln[e] = ln | ((int)(hi >> 32) << 24);  // repeat count - 1 in the top byte
+        if (mine && ((en.x >> 28) & 7) < ND_FEAS_SET)
+          for (int r = 0; r < s.R; r++) sh.dreq[e][r] = __ldg(&s.t_req[(size_t)en.y * s.R + r]);
       }
-      __syncwarp();
-      if (tid == 0) ts[0] += clock64() - c0;
-      if (lane < kDecWords) {  // every word is self-validating
-        unsigned long long lo, hi;
-        {
-          Spin spin;
-          do {
-            ld_relaxed_b128(rec0 + 2 * lane, lo, hi);
-          } while ((hi != (unsigned long long)seq) && !spin.expired(p, 8, (unsigned int)seq, (int)(lane)));
-        }
-        sh.dw[lane] = lo;
+      const unsigned int mb = __ballot_sync(0xffffffffu, mine), xb = __ballot_sync(0xffffffffu, ext);
+      if (lane == 0) {
+        sh.mine_bits[(e0 >> 5) + warp] = mb;
+        sh.ext_bits[(e0 >> 5) + warp] = xb;
       }
     }
     __syncthreads();
-    long long c1 = clock64();
-    if (tid < 32) {  // decode in parallel: lane r writes req[r], lanes 8/9 the trackers, lane 10 the scalars
-      const unsigned long long w0 = sh.dw[0];
-      const unsigned int bits = (unsigned int)((w0 >> 24) & 0xff);
-      Decision &d = sh.dec;
-      if (tid < KAI_MAX_RES) d.req[tid] = __longlong_as_double((long long)sh.dw[2 + tid]);
-      if (tid == 8 || tid == 9) {
-        const int k = tid - 8;
-        sh.trk[k].mn = __longlong_as_double((long long)sh.dw[10 + 2 * k]);
-        sh.trk[k].mx = __longlong_as_double((long long)sh.dw[11 + 2 * k]);
-        sh.trk[k].cnt_mn = (int)(unsigned int)(sh.dw[14 + k] & 0xffffffffu);
-        sh.trk[k].cnt_mx = (int)(unsigned int)(sh.dw[14 + k] >> 32);
-        sh.trk[k].dirty = (bits & (k == 0 ? DB_DIRTY0 : DB_DIRTY1)) ? 1 : 0;
-      }
-      if (tid == 10) {
-        sh.kind = (int)(w0 & 0xff);
-        d.res = (int)((w0 >> 8) & 0xff);
-        d.strategy = (int)((w0 >> 16) & 0xff);
-        sh.n_delta = (int)((w0 >> 32) & 0xffff);
-        sh.xbits = (int)((w0 >> 48) & 0xffff);
-        d.restricted = (sh.xbits & XB_RESTRICT) ? 1 : 0;
-        d.gpu_task = (bits & DB_GPU_TASK) ? 1 : 0;
-        d.best_effort = (bits & DB_BEST_EFFORT) ? 1 : 0;
-        d.pipeline_only = (bits & DB_PIPELINE_ONLY) ? 1 : 0;
-        sh.batching = (bits & DB_BATCHING) ? 1 : 0;
-        d.nominated = (int)(unsigned int)(sh.dw[1] & 0xffffffffu);
-        d.pred_class = (int)(unsigned int)(sh.dw[1] >> 32);
-        const int tk = d.res == KAI_RES_GPU ? 0 : 1;
-        d.mn = __longlong_as_double((long long)sh.dw[10 + 2 * tk]);
-        d.mx = __longlong_as_double((long long)sh.dw[11 + 2 * tk]);
-        d.task = -1;
-      }
-    }
-    __syncthreads();
-    long long c2 = clock64();
-    // ---- apply the node deltas that belong to this tile (loads in parallel, application in list order) ----
-    // Every scanner sees the whole list but owns ~1/scanners of it: the entries are classified in parallel (ballot bits
-    // per 32 entries: "mine", "extended") and only the set bits are walked, in list order.
-    const int nd = sh.n_delta;
-    if (nd > 0) {
-      const unsigned long long *dl = p.delta + (size_t)(seq & 1) * kMaxDelta * 2;
-      for (int e0 = 0; e0 < nd; e0 += blockDim.x) {
-        const int e = e0 + tid;
-        bool mine = false, ext = false;
-        if (e < nd) {
-          unsigned long long lo, hi;
-          if (LAUNCH) {
-            lo = (unsigned long long)lrec->dkey[e] | ((unsigned long long)lrec->dtask[e] << 32);
-            hi = (unsigned long long)seq | ((unsigned long long)lrec->dcount[e] << 32);
-          } else {
-            Spin spin;
-            do {
-              ld_relaxed_b128(dl + 2 * e, lo, hi);
-            } while (((unsigned int)hi != (unsigned int)seq) && !spin.expired(p, 9, (unsigned int)seq, (int)(e)));
-          }
-          int2 en = make_int2((int)(unsigned int)(lo & 0xffffffffu), (int)(unsigned int)(lo >> 32));
-          sh.delta[e] = en;
-          int ln = 0;
-          ext = en.x < 0;
-          mine = en.x >= 0 && tile_owns(tile, (unsigned int)(en.x & 0x0fffffff), ln) && ln < tile.count;
-          sh.dln[e] = ln | ((int)(hi >> 32) << 24);  // repeat count - 1 in the top byte
-          if (mine && ((en.x >> 28) & 7) < ND_FEAS_SET)
-            for (int r = 0; r < s.R; r++) sh.dreq[e][r] = __ldg(&s.t_req[(size_t)en.y * s.R + r]);
-        }
-        const unsigned int mb = __ballot_sync(0xffffffffu, mine), xb = __ballot_sync(0xffffffffu, ext);
-        if (lane == 0) {
-          sh.mine_bits[(e0 >> 5) + warp] = mb;
-          sh.ext_bits[(e0 >> 5) + warp] = xb;
-        }
-      }
-      __syncthreads();
-      const int n_words = (nd + 31) >> 5;
-      if (warp == 0 && lane < s.R) {
-        for (int w = 0; w < n_words; w++) {
-          unsigned int bits = sh.mine_bits[w];
-          while (bits) {
-            const int e = (w << 5) + __ffs((int)bits) - 1;
-            bits &= bits - 1;
-            int2 en = sh.delta[e];
-            const int ln = sh.dln[e] & 0xffffff, reps = ((unsigned int)sh.dln[e] >> 24) + 1;
-            const int code = (en.x >> 28) & 7;
-            if (code >= ND_FEAS_SET) {
-              if (lane == 0) tile.flags[ln] = code == ND_FEAS_SET ? (tile.flags[ln] | kTileFeas) : (tile.flags[ln] & ~kTileFeas);
-              continue;
-            }
-            for (int k = 0; k < reps; k++)
-              apply_delta_row(tile.I[lane * tile.npc + ln], tile.L[lane * tile.npc + ln], code, sh.dreq[e][lane]);
-          }
-        }
-      }
-      __syncthreads();
-      // extended entries, in list order: topology domain selection (each thread its own rows) and the per-domain
-      // score table (thread 0; the clearing BEGIN is the only step the others take part in)
-      bool any_ext = false;
+    const int n_words = (nd + 31) >> 5;
+    if (warp == 0 && lane < s.R) {
       for (int w = 0; w < n_words; w++) {
-        unsigned int bits = sh.ext_bits[w];
+        unsigned int bits = sh.mine_bits[w];
         while (bits) {
           const int e = (w << 5) + __ffs((int)bits) - 1;
           bits &= bits - 1;
-          any_ext = true;
-          const int2 en = sh.delta[e];
-          const int kind = (en.x >> 28) & 7;
-          const unsigned int a = (unsigned int)en.x & 0x0fffffffu, b = (unsigned int)en.y;
-          if (kind == EXT_SELECT || kind == EXT_SELECT_ROOT) {
-            const int slot = kind == EXT_SELECT ? (int)((a >> 8) & 7u) : (int)((a >> 16) & 7u);
-            const uint32_t bit = kTileDom >> slot;
-            for (int ln = tid; ln < tile.count; ln += blockDim.x) {
-              bool in;
-              if (kind == EXT_SELECT) {
-                in = tile.dom[((int)(a & 0xffu) - 1) * tile.npc + ln] == (int)b;
-              } else {
-                in = true;
-                for (int l = (int)(a & 0xff); l < (int)((a >> 8) & 0xff); l++)
-                  if (tile.dom[l * tile.npc + ln] < 0) in = false;
-              }
-              tile.flags[ln] = in ? (tile.flags[ln] | bit) : (tile.flags[ln] & ~bit);
-            }
-          } else if (kind == EXT_SCORE_BEGIN) {
-            __syncthreads();  // earlier EXT_SCORE writes of thread 0 precede the clearing
-            for (int i = tid; i < kDomBuckets; i += blockDim.x) sh.dom_bucket[i] = 255;
-            if (tid == 0) sh.pref_level = (int)a, sh.ext_dirty = 1;
-            __syncthreads();
-          } else if (kind == EXT_SCORE) {
-            if (tid == 0 && a < (unsigned int)kDomBuckets) sh.dom_bucket[a] = (unsigned char)b, sh.ext_dirty = 1;
-          } else if (kind == EXT_SCORE_END) {
-            if (tid == 0) sh.pref_level = -1, sh.ext_dirty = 1;
+          int2 en = sh.delta[e];
+          const int ln = sh.dln[e] & 0xffffff, reps = ((unsigned int)sh.dln[e] >> 24) + 1;
+          const int code = (en.x >> 28) & 7;
+          if (code >= ND_FEAS_SET) {
+            if (lane == 0) tile.flags[ln] = code == ND_FEAS_SET ? (tile.flags[ln] | kTileFeas) : (tile.flags[ln] & ~kTileFeas);
+            continue;
           }
+          for (int k = 0; k < reps; k++)
+            apply_delta_row(tile.I[lane * tile.npc + ln], tile.L[lane * tile.npc + ln], code, sh.dreq[e][lane]);
         }
       }
-      if (any_ext) __syncthreads();
     }
-    if (sh.xbits & (XB_SNAP_ALL | XB_SNAP_GPUFREE)) {  // common.FeasibleNodesForJob (feasible_nodes.go:11-26)
-      const bool all = (sh.xbits & XB_SNAP_ALL) != 0;
-      for (int ln = tid; ln < tile.count; ln += blockDim.x) {
-        bool in = all || tile.I[KAI_RES_GPU * tile.npc + ln] > 0 || tile.L[KAI_RES_GPU * tile.npc + ln] > 0;
-        tile.flags[ln] = in ? (tile.flags[ln] | kTileFeas) : (tile.flags[ln] & ~kTileFeas);
+    __syncthreads();
+    // extended entries, in list order: topology domain selection (each thread its own rows) and the per-domain
+    // score table (thread 0; the clearing BEGIN is the only step the others take part in)
+    bool any_ext = false;
+    for (int w = 0; w < n_words; w++) {
+      unsigned int bits = sh.ext_bits[w];
+      while (bits) {
+        const int e = (w << 5) + __ffs((int)bits) - 1;
+        bits &= bits - 1;
+        any_ext = true;
+        const int2 en = sh.delta[e];
+        const int kind = (en.x >> 28) & 7;
+        const unsigned int a = (unsigned int)en.x & 0x0fffffffu, b = (unsigned int)en.y;
+        if (kind == EXT_SELECT || kind == EXT_SELECT_ROOT) {
+          const int slot = kind == EXT_SELECT ? (int)((a >> 8) & 7u) : (int)((a >> 16) & 7u);
+          const uint32_t bit = kTileDom >> slot;
+          for (int ln = tid; ln < tile.count; ln += blockDim.x) {
+            bool in;
+            if (kind == EXT_SELECT) {
+              in = tile.dom[((int)(a & 0xffu) - 1) * tile.npc + ln] == (int)b;
+            } else {
+              in = true;
+              for (int l = (int)(a & 0xff); l < (int)((a >> 8) & 0xff); l++)
+                if (tile.dom[l * tile.npc + ln] < 0) in = false;
+            }
+            tile.flags[ln] = in ? (tile.flags[ln] | bit) : (tile.flags[ln] & ~bit);
+          }
+        } else if (kind == EXT_SCORE_BEGIN) {
+          __syncthreads();  // earlier EXT_SCORE writes of thread 0 precede the clearing
+          for (int i = tid; i < kDomBuckets; i += blockDim.x) sh.dom_bucket[i] = 255;
+          if (tid == 0) sh.pref_level = (int)a, sh.ext_dirty = 1;
+          __syncthreads();
+        } else if (kind == EXT_SCORE) {
+          if (tid == 0 && a < (unsigned int)kDomBuckets) sh.dom_bucket[a] = (unsigned char)b, sh.ext_dirty = 1;
+        } else if (kind == EXT_SCORE_END) {
+          if (tid == 0) sh.pref_level = -1, sh.ext_dirty = 1;
+        }
       }
-      __syncthreads();
     }
-    long long c3 = clock64();
-    const int kind = sh.kind;
-    if (kind == DK_DONE || ((volatile long long *)p.counters)[24] != 0) break;
-    if (LAUNCH && p.hot_in_smem && (kind == DK_SCAN || kind == DK_TOPK || kind == DK_MINMAX)) {
+    if (any_ext) __syncthreads();
+  }
+  if (sh.xbits & (XB_SNAP_ALL | XB_SNAP_GPUFREE)) {  // common.FeasibleNodesForJob (feasible_nodes.go:11-26)
+    const bool all = (sh.xbits & XB_SNAP_ALL) != 0;
+    for (int ln = tid; ln < tile.count; ln += blockDim.x) {
+      bool in = all || tile.I[KAI_RES_GPU * tile.npc + ln] > 0 || tile.L[KAI_RES_GPU * tile.npc + ln] > 0;
+      tile.flags[ln] = in ? (tile.flags[ln] | kTileFeas) : (tile.flags[ln] & ~kTileFeas);
+    }
+    __syncthreads();
+  }
+  long long c3 = clock64();
+  const int kind = sh.kind;
+  const bool done = kind == DK_DONE || ((volatile long long *)p.counters)[24] != 0;
+  if (!done) {
+    if (kind == DK_SCAN || kind == DK_TOPK || kind == DK_MINMAX) {
       // the sweep reads every row several times (top-M passes, repeat analysis): stage this scanner's block of g_tiles
       // in shared memory with one pass of independent 16-byte loads; deltas and row flags were applied to the
       // global copy above, nothing below writes the tile
@@ -1196,7 +940,7 @@ __device__ bool scanner_main(const ActionParams &p, const LaunchRec *lrec, unsig
       __syncthreads();
     }
     unsigned long long *slot = p.xbuf + (size_t)(seq & 1) * kMaxGrid * kSlotWords + (size_t)my * kSlotWords;
-    if (LAUNCH && !p.fused_in_kernel && kind == DK_SCAN && (sh.xbits & XB_FUSED_MM)) {
+    if (!p.fused_in_kernel && kind == DK_SCAN && (sh.xbits & XB_FUSED_MM)) {
       // the extremes of this row set were reduced by the MINMAX launch that precedes this one on the stream
       if (tid == 0) {
         const int k = sh.dec.res == KAI_RES_GPU ? 0 : 1;
@@ -1240,7 +984,7 @@ __device__ bool scanner_main(const ActionParams &p, const LaunchRec *lrec, unsig
         }
         __syncthreads();
         double g[4] = {DBL_MAX, 0.0, DBL_MAX, 0.0};
-        for (int c = tid; c < p.grid - 1; c += blockDim.x)
+        for (int c = tid; c < p.scanners; c += blockDim.x)
           for (int i = 0; i < 4; i++) {
             unsigned long long lo, hi;
             Spin spin;
@@ -1270,7 +1014,7 @@ __device__ bool scanner_main(const ActionParams &p, const LaunchRec *lrec, unsig
       }
     }
     if (kind == DK_SCAN && p.topm && !(sh.xbits & XB_SINGLE)) {
-      // ---- top-M answer straight into host memory (no relay reduction) ----
+      // ---- top-M answer into device lines (k_merge_cluster merges them; no last-CTA reduction) ----
       if (tid == 0) sh.fit_count = 0;
       __syncthreads();
       for (int m = 0; m < kTopM; m++) {
@@ -1282,7 +1026,7 @@ __device__ bool scanner_main(const ActionParams &p, const LaunchRec *lrec, unsig
         __syncthreads();
       }
       if (tid == 0) ts[4] += clock64() - c3;
-      unsigned long long *lines = p.h_list + ((size_t)(seq & 1) * kListScanners + (size_t)(p.scanner_base + my)) * kListLines * kListLineWords;
+      unsigned long long *lines = p.d_list + ((size_t)(seq & 1) * kListScanners + (size_t)my) * kListLines * kListLineWords;
       if (warp < kTopM) {
         double topo_term = 0.0;
         if (sh.pref_level >= 0 && sh.cands[warp].rank != kRankNone) {
@@ -1305,7 +1049,7 @@ __device__ bool scanner_main(const ActionParams &p, const LaunchRec *lrec, unsig
         }
         __syncthreads();
       }
-      unsigned long long *lines = p.h_list + ((size_t)(seq & 1) * kListScanners + (size_t)(p.scanner_base + my)) * kListLines * kListLineWords;
+      unsigned long long *lines = p.d_list + ((size_t)(seq & 1) * kListScanners + (size_t)my) * kListLines * kListLineWords;
       if (tid < kTopM) {
         const Cand c = sh.cands[tid];
         const uint32_t flags = sh.fit_count > kTopM ? LF_MORE : 0u;
@@ -1317,7 +1061,7 @@ __device__ bool scanner_main(const ActionParams &p, const LaunchRec *lrec, unsig
       Cand local = scan_tile(tile, sh.dec, s, sh_warp, nullptr, 0, nullptr, sh.xbits, sh.pref_level, sh.dom_bucket);
       long long c4 = clock64();
       if (tid == 0) ts[4] += c4 - c3;
-      if (warp == 0) publish_candidate(sh.trk, tile, sh.dec, local, slot, seq & 0xffffffu, sh.batching, false, my == 0 ? p.counters + 40 : nullptr);
+      if (warp == 0) publish_candidate(sh.trk, tile, sh.dec, local, slot, seq & 0xffffffu, sh.batching, my == 0 ? p.counters + 40 : nullptr);
     } else if (kind == DK_MINMAX) {
       double mn[2] = {DBL_MAX, DBL_MAX}, mx[2] = {0, 0};
       for (int ln = tid; ln < tile.count; ln += blockDim.x)
@@ -1394,24 +1138,15 @@ __device__ bool scanner_main(const ActionParams &p, const LaunchRec *lrec, unsig
       ts[5] += c5 - c3;  // scan + publish
       ts[6]++;
     }
-    seq++;
     __syncthreads();
-    if (LAUNCH) {
-      wrote_answer = true;
-      break;
-    }
   }
-  if (LAUNCH && tid == 0 && my == 0)  // launches of one action follow each other on the stream: plain accumulation
+  if (tid == 0 && my == 0)  // launches of one action follow each other on the stream: plain accumulation
     for (int i = 0; i < 7; i++) p.counters[32 + i] += ts[i];
-  if (LAUNCH) {
-    if (sh.ext_dirty) {  // preferred-level score table of this scanner: back to its global copy
-      for (int i = tid; i < kDomBuckets; i += blockDim.x) gstate[16 + i] = sh.dom_bucket[i];
-      if (tid == 0) *(int *)gstate = sh.pref_level;
-    }
-    if (wrote_answer) return sh.kind != DK_FLUSH;
+  if (sh.ext_dirty) {  // preferred-level score table of this scanner: back to its global copy
+    for (int i = tid; i < kDomBuckets; i += blockDim.x) gstate[16 + i] = sh.dom_bucket[i];
+    if (tid == 0) *(int *)gstate = sh.pref_level;
   }
-  if (!LAUNCH && tid == 0 && my == 0)
-    for (int i = 0; i < 7; i++) p.counters[32 + i] = ts[i];
+  if (!done) return kind != DK_FLUSH;
   // ---- DONE: write the tile back to the session tables ----
   for (int ln = tid; ln < tile.count; ln += blockDim.x) {
     int n = tile.node[ln];
@@ -1424,265 +1159,13 @@ __device__ bool scanner_main(const ActionParams &p, const LaunchRec *lrec, unsig
 }
 
 // =============================================================================================
-// sequencer CTA
-// =============================================================================================
-__device__ void sequencer_main(const ActionParams &p, unsigned char *smem, Ctl &ctl, Seq &seq) {
-  const DevSnap &s = p.s;
-  const int tid = threadIdx.x, lane = tid & 31;
-  if (tid == 0) {
-    unsigned char *h = p.hot_in_smem ? smem : s.hot_global;
-    auto take_from = [](unsigned char *&base, size_t bytes) {
-      unsigned char *r = base;
-      base += (bytes + 15) & ~(size_t)15;
-      return r;
-    };
-    Replica &rp = seq.rp;
-    rp.q_alloc = (double *)take_from(h, sizeof(double) * QR * s.Q);
-    rp.q_alloc_np = (double *)take_from(h, sizeof(double) * QR * s.Q);
-    rp.qkey = (QKey *)take_from(h, sizeof(QKey) * s.Q);
-    rp.leaf_head = (int *)take_from(h, sizeof(int) * s.Q);
-    rp.leaf_end = (int *)take_from(h, sizeof(int) * s.Q);
-    rp.ovl_len = (int *)take_from(h, sizeof(int) * s.Q);
-    rp.child_len = (int *)take_from(h, sizeof(int) * s.Q);
-    rp.child_heap = (int *)take_from(h, sizeof(int) * s.Q);
-    rp.root_heap = (int *)take_from(h, sizeof(int) * (s.n_top + 1));
-    rp.qn_flags = (unsigned char *)take_from(h, s.Q);
-    rp.touched = (unsigned int *)take_from(h, sizeof(unsigned int) * ((s.J + 31) / 32 + 1));
-    // cold state = the session arrays themselves
-    rp.t_status = s.t_status;
-    rp.t_node = s.t_node;
-    rp.t_node_status = s.t_node_status;
-    rp.t_virtual = s.t_virtual;
-    rp.ps_active_alloc = s.ps_cnt0;
-    rp.ps_pending = s.ps_cnt0 + s.S;
-    rp.ps_pipelined = s.ps_cnt0 + 2 * s.S;
-    rp.j_req = s.j_req;
-    rp.j_req_valid = s.j_req_valid;
-    rp.j_key = s.j_key0;
-    rp.leaf_heap = s.leaf_sorted;
-    rp.ops = s.ops;
-    rp.tta = s.tta;
-    rp.ps_order = s.ps_order;
-    seq.s = &p.s;
-    seq.cfg = &p.cfg;
-    seq.p = &p;
-    seq.delta_base = p.delta;
-    seq.host_backend = nullptr;
-    seq.tile = nullptr;
-    seq.ctl = &ctl;
-    seq.n_ops = 0;
-    seq.ops_cap = p.ops_cap;
-    seq.root_len = 0;
-    seq.batching = p.batching;
-    seq.is_cta0 = true;
-    seq.pods_placed = seq.pods_evicted = seq.sweeps = seq.nodes_scanned = seq.n_visits = 0;
-    seq.minmax_exchanges = seq.batched = 0;
-    seq.visits = p.visits;
-    seq.visits_cap = p.visits_cap;
-    seq.error = 0;
-    seq.t_pop = seq.t_prep = seq.t_scan = seq.t_xchg = seq.t_apply = seq.t_finish = seq.t_init = 0;
-    seq.t_key = seq.n_key = seq.t_tta = seq.t_heap = 0;
-    ctl.trk[0].dirty = ctl.trk[1].dirty = 1;
-    ctl.trk[0].mn = ctl.trk[1].mn = DBL_MAX;
-    ctl.trk[0].mx = ctl.trk[1].mx = 0;
-    ctl.trk[0].cnt_mn = ctl.trk[0].cnt_mx = ctl.trk[1].cnt_mn = ctl.trk[1].cnt_mx = 0;
-    ctl.batch.valid = 0;
-    for (int r = 0; r < KAI_MAX_RES; r++) ctl.dec.req[r] = 0;
-    ctl.dec.pipeline_only = ctl.dec.res = ctl.dec.strategy = ctl.dec.gpu_task = ctl.dec.best_effort = 0;
-    ctl.dec.nominated = ctl.dec.pred_class = -1;
-    ctl.dec.task = -1;
-    ctl.ctx_job = ctl.ctx_ps = -1;
-    ctl.ctx_fresh = ctl.ctx_queue = ctl.ctx_preempt = ctl.ctx_base = 0;
-    ctl.seq = p.seq0;
-    ctl.n_delta = 0;
-    ctl.last_dcount = 0;
-    ctl.xbits = 0;
-    ctl.dec.restricted = 0;
-    ctl.stop = 0;
-  }
-  __syncthreads();
-  long long tk0 = clock64();
-  {
-    Replica &rp = seq.rp;
-    for (int i = tid; i < QR * s.Q; i += blockDim.x) {
-      rp.q_alloc[i] = s.q_alloc[i];
-      rp.q_alloc_np[i] = s.q_alloc_np[i];
-    }
-    for (int i = tid; i < s.Q; i += blockDim.x) {
-      int b = s.q_job_begin[i];
-      rp.leaf_head[i] = b;
-      rp.leaf_end[i] = b + (s.q_nchildren[i] == 0 ? s.leaf_count[i] : 0);
-      rp.ovl_len[i] = 0;
-      rp.child_len[i] = 0;
-      rp.qn_flags[i] = 0;
-      rp.qkey[i].valid = 0;
-    }
-    for (int i = tid; i < (s.J + 31) / 32 + 1; i += blockDim.x) rp.touched[i] = 0;
-  }
-  __syncthreads();
-  if (tid >= 32) return;  // the sequencer proper is warp 0
-  if (lane == 0) {
-    seq_init_job_order(seq);
-    seq.t_init = clock64() - tk0;
-  }
-  __syncwarp();
-
-  // ---- allocate action main loop (actions/allocate/allocate.go:46-111) ----
-  for (;;) {
-    if (lane == 0) {
-      long long tk = clock64();
-      int job = pop_next_job(seq);
-      ctl.job = job;
-      ctl.n_items = 0;
-      ctl.job_ok = 0;
-      if (job >= 0) {
-        seq.n_ops = 0;
-        long long tkt = clock64();
-        seq.t_heap += tkt - tk;
-        // job context: queue, preemptibility and (single-podset jobs) the podset counters
-        const JobRec rec = s.jrec[job];
-        ctl.ctx_job = job;
-        ctl.ctx_queue = __ldg(&s.j_queue[job]);
-        ctl.ctx_preempt = (__ldg(&s.j_flags[job]) & KAI_JOB_PREEMPTIBLE) ? 1 : 0;
-        ctl.ctx_fresh = (!job_touched(seq, job) && rec.n_tta >= 0) ? 1 : 0;
-        ctl.ctx_ps = -1;
-        if (rec.n_podsets == 1) {
-          if (!job_touched(seq, job)) {
-            ctl.ctx_cnt[0] = rec.cnt[0];
-            ctl.ctx_cnt[1] = rec.cnt[1];
-            ctl.ctx_cnt[2] = rec.cnt[2];
-          } else {
-            for (int w = 0; w < 3; w++) ctl.ctx_cnt[w] = seq.rp.ps_active_alloc[(size_t)w * s.S + rec.ps0];
-          }
-          ctl.ctx_ps = rec.ps0;
-        }
-        // common/allocate.go:20-36 AllocateJob
-        int n;
-        double req[QR] = {0, 0, 0};
-        if (ctl.ctx_fresh) {  // GetTasksToAllocate = tasks [tb, tb + n_tta), request sum precomputed
-          n = rec.n_tta;
-          ctl.ctx_base = rec.tb;
-          for (int r = 0; r < QR; r++) req[r] = rec.req0[r];
-          for (int k = 0; k < n; k++) prefetch_l1(s.t_req + (size_t)(rec.tb + k) * s.R);
-        } else {
-          n = tasks_to_allocate(seq, job, true, nullptr);
-          ctl.ctx_base = -1;
-          for (int k = 0; k < n; k++)
-            for (int r = 0; r < QR; r++) req[r] = __dadd_rn(req[r], __ldg(&s.t_req[(size_t)seq.rp.tta[k] * s.R + r]));
-        }
-        seq.t_tta += clock64() - tkt;
-        if (!over_capacity(seq, job, req)) {
-          // tasks_to_allocate already emits tasks grouped in PodSetOrderFn order, which is the order
-          // allocateSubGroupSetOnNodes/allocatePodSet visit them in (common/allocate.go:62-119)
-          ctl.n_items = n;
-          ctl.job_ok = 1;
-        }
-      }
-      if (seq.error || ((volatile long long *)p.counters)[24] != 0) ctl.stop = 1;
-      seq.t_pop += clock64() - tk;
-    }
-    __syncwarp();
-    if (ctl.job < 0 || ctl.stop) break;
-    bool job_success = ctl.job_ok != 0;
-    if (job_success) {
-      const int n_items = ctl.n_items;
-      for (int k = 0; k < n_items; k++) {
-        if (lane == 0) {
-          long long tk = clock64();
-          int t = ctl.ctx_base >= 0 ? ctl.ctx_base + k : seq.rp.tta[k];
-          ctl.item_ok = seq_prepare_task(seq, t, ctl.job) ? 1 : 0;
-          if (ctl.item_ok && ctl.use_batch) seq_apply_batched(seq, t);
-          if (ctl.need_minmax) seq.minmax_exchanges++;
-          seq.t_prep += clock64() - tk;
-        }
-        __syncwarp();
-        if (!ctl.item_ok) {
-          job_success = false;
-          break;
-        }
-        if (ctl.use_batch) continue;  // placed without a sweep (same-node batching)
-        long long tk1 = clock64();
-        if (ctl.need_minmax) {
-          seq_publish(p, ctl, DK_MINMAX);
-          seq_gather_minmax(p, ctl);
-        }
-        seq_publish(p, ctl, DK_SCAN);
-        seq_gather_candidates(p, ctl);
-        if (lane == 0) {
-          long long tk3 = clock64();
-          seq_apply_winner(seq, ctl.dec.task);
-          long long tk4 = clock64();
-          seq.t_xchg += tk3 - tk1;
-          seq.t_apply += tk4 - tk3;
-        }
-        __syncwarp();
-        if (!ctl.item_ok) {
-          job_success = false;
-          break;
-        }
-      }
-    }
-    if (lane == 0) {
-      long long tk = clock64();
-      int job = ctl.job;
-      if (job_success) {
-        if (should_pipeline_job(seq, job)) stmt_convert_all_allocated_to_pipelined(seq, job);
-        stmt_commit(seq);
-        record_visit(seq, job, 1);
-        if (has_tasks_to_allocate(seq, job)) push_job(seq, job);
-      } else {
-        stmt_rollback(seq, 0);  // Discard (statement.go:522-534)
-        record_visit(seq, job, 0);
-      }
-      if (ctl.ctx_ps >= 0)  // write the podset counters of the job back to the session state
-        for (int w = 0; w < 3; w++) seq.rp.ps_active_alloc[(size_t)w * s.S + ctl.ctx_ps] = ctl.ctx_cnt[w];
-      ctl.ctx_ps = -1;
-      ctl.ctx_job = -1;
-      ctl.ctx_fresh = 0;
-      if (seq.error) ctl.stop = 1;
-      seq.t_finish += clock64() - tk;
-    }
-    __syncwarp();
-    if (ctl.stop) break;
-  }
-  // ---- DONE record (carries the last deltas), write back the hot per-queue state and the counters ----
-  seq_publish(p, ctl, DK_DONE);
-  for (int i = lane; i < QR * s.Q; i += 32) {
-    s.q_alloc[i] = seq.rp.q_alloc[i];
-    s.q_alloc_np[i] = seq.rp.q_alloc_np[i];
-  }
-  if (lane == 0) {
-    p.counters[0] = seq.n_visits;
-    p.counters[1] = seq.sweeps;
-    p.counters[2] = seq.nodes_scanned;
-    p.counters[3] = seq.pods_placed;
-    p.counters[4] = seq.pods_evicted;
-    p.counters[5] = seq.minmax_exchanges;
-    p.counters[6] = seq.error;
-    p.counters[7] = ctl.seq + 1;
-    p.counters[8] = seq.t_init;
-    p.counters[9] = seq.t_pop;
-    p.counters[10] = seq.t_prep;
-    p.counters[11] = seq.t_key;
-    p.counters[12] = seq.t_xchg;
-    p.counters[13] = seq.t_apply;
-    p.counters[14] = seq.t_finish;
-    p.counters[15] = seq.batched;
-    p.counters[16] = seq.n_key;
-    p.counters[17] = seq.t_tta;
-    p.counters[18] = seq.t_heap;
-  }
-}
-
-// =============================================================================================
-// relay CTA (host-sequenced mode): forwards the host's decision records and node deltas from pinned mapped
-// host memory (one PCIe reader for the whole GPU) into the device-side record buffer the scanners poll
+// the last CTA of a launch
 // =============================================================================================
 // Reduce the scanners' answers for record `seq` on the GPU and write ONE 64-byte line to host memory (a host
 // core pays ~80 ns per GPU-written cache line it reads; 147 lines per sweep were the bottleneck).
-__device__ void relay_reduce(const ActionParams &p, int kind, unsigned int seq) {
+__device__ void reduce_answers(const ActionParams &p, int kind, unsigned int seq) {
   const int lane = threadIdx.x & 31;
-  const int n = p.grid - 1;
+  const int n = p.scanners;
   if (kind == DK_SCAN || kind == DK_FLUSH) {
     const unsigned long long *buf = p.xbuf + (size_t)(seq & 1) * kMaxGrid * kSlotWords;
     const unsigned int tag = seq & 0xffffffu;
@@ -1793,7 +1276,7 @@ __device__ void relay_reduce(const ActionParams &p, int kind, unsigned int seq) 
             cmx[k] += ocmx;
         }
       }
-    if (lane == 0 && p.mm_result) {  // launch transport: the next launch (XB_FUSED_MM sweep) reads the extremes on the device
+    if (lane == 0) {  // the next launch (XB_FUSED_MM sweep) reads the extremes on the device
       for (int k = 0; k < 2; k++) {
         p.mm_result[2 * k] = cmn[k] > 0 ? gmn[k] : DBL_MAX;
         p.mm_result[2 * k + 1] = cmx[k] > 0 ? gmx[k] : 0.0;
@@ -1812,243 +1295,22 @@ __device__ void relay_reduce(const ActionParams &p, int kind, unsigned int seq) 
   __syncwarp();
 }
 
-__device__ void relay_main(const ActionParams &p) {
-  if (threadIdx.x >= 32) return;
-  const int lane = threadIdx.x;
-  unsigned int seq = p.seq0;
-  long long acc_fwd = 0, acc_wait = 0, acc_red = 0, n_rec = 0;
-  for (;;) {
-    const unsigned long long *hrec = p.h_rec + (size_t)(seq & 1) * kDecWords * 2;
-    const unsigned long long *hdl = p.h_delta + (size_t)(seq & 1) * kMaxDelta * 2;
-    unsigned long long *drec = p.dbuf + (size_t)(seq & 1) * kDecWords * 2;
-    unsigned long long *ddl = p.delta + (size_t)(seq & 1) * kMaxDelta * 2;
-    // lanes 0..15 poll the record words, lanes 16..31 speculatively the first 16 deltas: one PCIe round trip
-    const unsigned long long *src = lane < kDecWords ? hrec + 2 * lane : hdl + 2 * (lane - kDecWords);
-    unsigned long long lo = 0, hi = 0;
-    Spin spin;
-    for (;;) {
-      ld_relaxed_sys_b128(src, lo, hi);
-      unsigned int got = __ballot_sync(0xffffffffu, hi == (unsigned long long)seq);
-      if ((got & 0xffffu) == 0xffffu || spin.expired(p, 10, seq, lane)) break;
-    }
-    long long tr0 = clock64();
-    unsigned long long w0 = __shfl_sync(0xffffffffu, lo, 0);
-    const int kind = (int)(w0 & 0xff);
-    const int nd = (int)((w0 >> 32) & 0xffff);
-    // deltas first, then the record words (every word is self-validating, so no ordering is required)
-    for (int e = lane - kDecWords; e < nd; e += 32) {
-      if (e < 0) continue;
-      unsigned long long dlo = lo, dhi = hi;
-      if (e >= 32 - kDecWords || (unsigned int)dhi != seq) {
-        Spin sp2;
-        do {
-          ld_relaxed_sys_b128(hdl + 2 * e, dlo, dhi);
-        } while ((unsigned int)dhi != seq && !sp2.expired(p, 11, seq, e));
-      }
-      st_relaxed_b128(ddl + 2 * e, dlo, dhi);
-    }
-    __syncwarp();
-    if (lane < kDecWords) st_relaxed_b128(drec + 2 * lane, lo, hi);
-    __syncwarp();
-    if (lane == 0) ((volatile long long *)p.counters)[23] = ((long long)kind << 32) | seq;  // last forwarded record
-    if (kind == DK_DONE || ((volatile long long *)p.counters)[24] != 0) break;
-    long long tr1 = clock64();
-    const unsigned int xb = (unsigned int)((w0 >> 48) & 0xffff);
-    if (!((p.topm && kind == DK_SCAN && !(xb & XB_SINGLE)) || kind == DK_TOPK)) relay_reduce(p, kind, seq);
-    long long tr2 = clock64();
-    acc_fwd += tr1 - tr0;
-    acc_red += tr2 - tr1;
-    n_rec++;
-    seq++;
-  }
-  if (lane == 0) {
-    p.counters[20] = acc_fwd;
-    p.counters[21] = acc_red;
-    p.counters[22] = n_rec;
-  }
-}
-
 // =============================================================================================
-// the kernel
+// list answers: merge of the scanners' top-M candidates
 // =============================================================================================
-__global__ void __launch_bounds__(kThreads, 1) k_action(const __grid_constant__ ActionParams p) {
-  extern __shared__ __align__(16) unsigned char smem[];
-  __shared__ Ctl ctl;
-  __shared__ Tile tile;
-  __shared__ Seq seq;
-  __shared__ ScanShared scan_sh;
-  __shared__ Cand sh_warp[kThreads / 32];
-  __shared__ double sh_d[(kThreads / 32) * 8];
-  __shared__ int sh_i[(kThreads / 32) * 4];
-  if (blockIdx.x == 0) {
-    if (p.mode != 0)
-      relay_main(p);
-    else
-      sequencer_main(p, smem, ctl, seq);
-  } else
-    scanner_main<false>(p, nullptr, smem, sh_warp, sh_d, sh_i, scan_sh, tile);
-}
-
-
-// =============================================================================================
-// launch transport: one kernel launch per decision record
-// =============================================================================================
-// Last CTA of a list launch: merge the top-M answers of all scanners (device lines, layout of h_list) into one list in
-// key order, cut it where an unseen row could be better (the best "last reported key" among scanners that have more
-// fitting rows than they reported — the rule HostBackend::gather_list applies), and write the usable prefix as
-// 48-byte entries {score, meta, Ig, Lg, Ic, Lc} + one header word to host memory: the host reads one contiguous list
-// instead of scanners x (1 + M) cache lines.
 // Integer sort keys of a candidate: h = ~bits(score) (scores are sums of non-negative terms, so ascending h is descending
 // score), l = rank << 32 | source (scanner * kTopM + m); an empty slot is all ones in both and sorts last.
 constexpr int kMergeThreads = 1024;  // one candidate per thread: scanners x kTopM <= 1024
-constexpr size_t kMergeSmemBytes = (size_t)kMergeThreads * 8 * (2 + kCEntryWords);
 __device__ __forceinline__ bool mk_before(unsigned long long ah, unsigned long long al, unsigned long long bh, unsigned long long bl) {
   return ah < bh || (ah == bh && al < bl);
 }
-// Merge kernel of the launch transport (one CTA, launched right after a list sweep on the same stream): sorts the
-// scanners' top-M candidates by (score desc, name rank asc) — bitonic network, partner exchange by warp shuffle below
-// 32 lanes and through shared memory above —, cuts the list where an unseen row could be better (the best "last
-// reported key" among scanners that have more fitting rows than they reported: the rule HostBackend::gather_list
-// applies) and streams the usable prefix as 48-byte entries {score, meta, Ig, Lg, Ic, Lc} + one header word to host
-// memory: the host reads one contiguous list instead of scanners x (1 + M) cache lines.
-__global__ void __launch_bounds__(kMergeThreads, 1) k_merge(const __grid_constant__ ActionParams p, unsigned int seq, int with_payload) {
-  extern __shared__ __align__(16) unsigned char dyn_smem[];  // kMergeSmemBytes: exchange planes + staged entries
-  unsigned long long *xh = (unsigned long long *)dyn_smem, *xl = xh + kMergeThreads, *stage = xl + kMergeThreads;
-  __shared__ unsigned long long cut_h[kMergeThreads / 32];
-  __shared__ unsigned int cut_r[kMergeThreads / 32];
-  __shared__ int n_ok[kMergeThreads / 32];
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int n_scan = p.grid - 1;
-  const int n_c = n_scan * kTopM;
-  const unsigned long long *base = p.h_list + (size_t)(seq & 1) * kListScanners * kListLines * kListLineWords;
-  const long long t0 = clock64();
-  // ---- my candidate; the cut key of my scanner (lanes 4c .. 4c+3 hold scanner c) ----
-  unsigned long long h = ~0ull, l = ~0ull;
-  bool more = false;
-  if (tid < n_c) {
-    const int c = tid / kTopM, m = tid % kTopM;
-    const unsigned long long *lines = base + (size_t)(p.scanner_base + c) * kListLines * kListLineWords;
-    const uint4 v = __ldcg((const uint4 *)(lines + 2 * m));  // written by the previous launch: plain (overlappable) loads
-    const unsigned long long lo = (unsigned long long)v.x | ((unsigned long long)v.y << 32);
-    const unsigned long long hi = (unsigned long long)v.z | ((unsigned long long)v.w << 32);
-    const uint32_t rank = (uint32_t)(hi & 0xffffffu);
-    more = (((uint32_t)(hi >> 32) & 0xffu) & LF_MORE) != 0;
-    if (rank != kRankNone) {
-      h = ~lo;
-      l = ((unsigned long long)rank << 32) | (unsigned long long)tid;
-    }
-  }
-  // cut candidate of a scanner: its last reported key when it has more rows; the best of those over all scanners
-  static_assert(kTopM == 4, "the group reductions below assume 4 candidates per scanner");
-  const unsigned int grp = 0xfu << (lane & ~3);
-  const bool any_more = (__ballot_sync(0xffffffffu, more) & grp) != 0;
-  const unsigned int real = __ballot_sync(0xffffffffu, l != ~0ull) & grp;
-  unsigned long long ch = ~0ull;  // candidate cut key held by the lane of the group's last real entry
-  unsigned int cr = kRankNone;
-  if (any_more && real && lane == 31 - __clz((int)real)) {
-    ch = h;
-    cr = (unsigned int)(l >> 32);
-  }
-  for (int o = 16; o > 0; o >>= 1) {
-    const unsigned long long oh = __shfl_xor_sync(0xffffffffu, ch, o);
-    const unsigned int orr = __shfl_xor_sync(0xffffffffu, cr, o);
-    if (orr != kRankNone && (cr == kRankNone || oh < ch || (oh == ch && orr < cr))) {
-      ch = oh;
-      cr = orr;
-    }
-  }
-  if (lane == 0) {
-    cut_h[warp] = ch;
-    cut_r[warp] = cr;
-  }
-  const long long t1 = clock64();
-  // ---- bitonic sort, one element per thread ----
-  for (int k = 2; k <= kMergeThreads; k <<= 1)
-    for (int j = k >> 1; j > 0; j >>= 1) {
-      unsigned long long oh, ol;
-      if (j < 32) {
-        oh = __shfl_xor_sync(0xffffffffu, h, j);
-        ol = __shfl_xor_sync(0xffffffffu, l, j);
-      } else {
-        xh[tid] = h;
-        xl[tid] = l;
-        __syncthreads();
-        oh = xh[tid ^ j];
-        ol = xl[tid ^ j];
-        __syncthreads();
-      }
-      const bool lower = (tid & j) == 0;        // I keep the earlier key of the pair when the run ascends
-      const bool up = (tid & k) == 0;
-      const bool other_first = mk_before(oh, ol, h, l);
-      const bool take = (lower == up) ? other_first : mk_before(h, l, oh, ol);
-      if (take) {
-        h = oh;
-        l = ol;
-      }
-    }
-  __syncthreads();
-  const long long t2 = clock64();
-  unsigned long long gh = ~0ull;
-  unsigned int gr = kRankNone;
-  for (int w = 0; w < kMergeThreads / 32; w++) {
-    const unsigned long long oh = cut_h[w];
-    const unsigned int orr = cut_r[w];
-    if (orr != kRankNone && (gr == kRankNone || oh < gh || (oh == gh && orr < gr))) {
-      gh = oh;
-      gr = orr;
-    }
-  }
-  const bool have_cut = gr != kRankNone;
-  // ---- usable prefix: real entries that are not worse than the cut (sorted: they form a prefix) ----
-  const unsigned int my_rank = (unsigned int)(l >> 32);
-  const bool ok = l != ~0ull && (!have_cut || h < gh || (h == gh && my_rank <= gr));
-  const unsigned int okb = __ballot_sync(0xffffffffu, ok);
-  if (lane == 0) n_ok[warp] = __popc(okb);
-  __syncthreads();
-  int n_out = 0;
-  for (int w = 0; w < kMergeThreads / 32; w++) n_out += n_ok[w];
-  unsigned long long *out = p.h_clist + (size_t)(seq & 1) * kCListWords;
-  if (tid < n_out) {
-    const int src = (int)(l & 0xffffffffu);
-    const int c = src / kTopM, m = src % kTopM;
-    const unsigned long long *lines = base + (size_t)(p.scanner_base + c) * kListLines * kListLineWords;
-    const uint4 v = __ldcg((const uint4 *)(lines + 2 * m));
-    uint4 pw[4];
-#pragma unroll
-    for (int q = 0; q < 4; q++) pw[q] = make_uint4(0, 0, 0, 0);
-    if (with_payload) {
-      const unsigned long long *pl = lines + (size_t)(1 + m) * kListLineWords;
-#pragma unroll
-      for (int q = 0; q < 4; q++) pw[q] = __ldcg((const uint4 *)(pl + 2 * q));
-    }
-    unsigned long long *e = stage + (size_t)tid * kCEntryWords;
-    e[0] = (unsigned long long)v.x | ((unsigned long long)v.y << 32);
-    e[1] = (unsigned long long)v.z | ((unsigned long long)v.w << 32);
-#pragma unroll
-    for (int q = 0; q < 4; q++) e[2 + q] = (unsigned long long)pw[q].x | ((unsigned long long)pw[q].y << 32);
-  }
-  __syncthreads();
-  const long long t3 = clock64();
-  // one linear stream of 16-byte stores: consecutive threads write consecutive addresses (full-size PCIe packets)
-  const int n16 = (n_out * kCEntryWords) / 2;
-  for (int i = tid; i < n16; i += kMergeThreads) st_relaxed_sys_b128(out + 2 + 2 * (size_t)i, stage[2 * i], stage[2 * i + 1]);
-  __syncthreads();
-  const long long t4 = clock64();
-  if (tid == 0) {
-    __threadfence_system();  // the entries (ordered before by the barrier) reach host memory before the header
-    st_relaxed_sys_b128(out, (unsigned long long)(unsigned int)n_out | (have_cut ? (1ull << 31) : 0ull), (unsigned long long)seq);
-    const long long t5 = clock64();
-    p.counters[44] += t5 - t0;
-    p.counters[45] += 1;
-    p.counters[46] += t2 - t1;  // sort
-    p.counters[47] += t4 - t3;  // stream to the host
-    p.counters[43] += t5 - t4;  // fence + header
-    p.counters[39] += t1 - t0;  // candidate loads + cut
-    p.counters[31] += t3 - t2;  // prefix + payload loads
-  }
-}
-
-// The same merge on a thread-block cluster (Hopper: 4 CTAs x 256 threads on 4 SMs, one candidate per thread): the
+// Merge kernel, launched right after a list sweep on the same stream: sorts the scanners' top-M candidates (device lines
+// of d_list) by (score desc, name rank asc) with a bitonic network, cuts the list where an unseen row could be better
+// (the best "last reported key" among scanners that have more fitting rows than they reported) and streams the usable
+// prefix as 48-byte entries {score, meta, Ig, Lg, Ic, Lc} + one header word to host memory: the host reads one
+// contiguous list instead of scanners x (1 + M) cache lines.
+//
+// It runs on a thread-block cluster (Hopper: 4 CTAs x 256 threads on 4 SMs, one candidate per thread): the
 // 55-step network is bound by instruction issue, so four SMs share it instead of one.  Partner exchange: warp shuffle
 // below 32 lanes, the CTA's shared memory below 256, the partner CTA's shared memory (distributed shared memory,
 // cluster.map_shared_rank) for the three steps with j >= 256; every CTA streams its own quarter of the sorted prefix to
@@ -2070,15 +1332,15 @@ __global__ void __cluster_dims__(kMergeCtas, 1, 1) __launch_bounds__(kMergeCtaTh
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const unsigned int crank = cluster.block_rank();
   const int g = (int)crank * kMergeCtaThreads + tid;  // my position in the network
-  const int n_scan = p.grid - 1;
+  const int n_scan = p.scanners;
   const int n_c = n_scan * kTopM;
-  const unsigned long long *base = p.h_list + (size_t)(seq & 1) * kListScanners * kListLines * kListLineWords;
+  const unsigned long long *base = p.d_list + (size_t)(seq & 1) * kListScanners * kListLines * kListLineWords;
   const long long t0 = clock64();
   unsigned long long h = ~0ull, l = ~0ull;
   bool more = false;
   if (g < n_c) {
     const int c = g / kTopM, m = g % kTopM;
-    const unsigned long long *lines = base + (size_t)(p.scanner_base + c) * kListLines * kListLineWords;
+    const unsigned long long *lines = base + (size_t)c * kListLines * kListLineWords;
     const uint4 v = __ldcg((const uint4 *)(lines + 2 * m));
     const unsigned long long lo = (unsigned long long)v.x | ((unsigned long long)v.y << 32);
     const unsigned long long hi = (unsigned long long)v.z | ((unsigned long long)v.w << 32);
@@ -2187,7 +1449,7 @@ __global__ void __cluster_dims__(kMergeCtas, 1, 1) __launch_bounds__(kMergeCtaTh
   if (g < n_out) {
     const int src = (int)(l & 0xffffffffu);
     const int c = src / kTopM, m = src % kTopM;
-    const unsigned long long *lines = base + (size_t)(p.scanner_base + c) * kListLines * kListLineWords;
+    const unsigned long long *lines = base + (size_t)c * kListLines * kListLineWords;
     const uint4 v = __ldcg((const uint4 *)(lines + 2 * m));
     uint4 pw[4];
 #pragma unroll
@@ -2223,7 +1485,9 @@ __global__ void __cluster_dims__(kMergeCtas, 1, 1) __launch_bounds__(kMergeCtaTh
   }
 }
 
-__global__ void __launch_bounds__(kThreads) k_record(const __grid_constant__ ActionParams p, const __grid_constant__ LaunchRec rec) {
+// Asks for 5 resident CTAs per SM, which caps the budget at 102 registers.  Left to its default, ptxas settles on 80
+// registers and spills about 300 B per thread to local memory; with the bound it uses 96 registers and no spills.
+__global__ void __launch_bounds__(kThreads, 5) k_record(const __grid_constant__ ActionParams p, const __grid_constant__ LaunchRec rec) {
   extern __shared__ __align__(16) unsigned char smem[];  // merge keys of the last CTA
   __shared__ Tile tile;
   __shared__ ScanShared scan_sh;
@@ -2231,9 +1495,9 @@ __global__ void __launch_bounds__(kThreads) k_record(const __grid_constant__ Act
   __shared__ double sh_d[(kThreads / 32) * 8];
   __shared__ int sh_i[(kThreads / 32) * 4];
   __shared__ int is_last;
-  const bool answers = scanner_main<true>(p, &rec, smem, sh_warp, sh_d, sh_i, scan_sh, tile);
+  const bool answers = scanner_main(p, &rec, smem, sh_warp, sh_d, sh_i, scan_sh, tile);
   if (!answers) return;
-  // list answers (top-M lines in device memory) are merged by k_merge, the next launch on the stream
+  // list answers (top-M lines in device memory) are merged by k_merge_cluster, the next launch on the stream
   if (scan_sh.kind == DK_TOPK || (scan_sh.kind == DK_SCAN && p.topm && !(scan_sh.xbits & XB_SINGLE))) return;
   // ---- the last CTA to finish reduces the answers of all scanners and writes the result to host memory ----
   __threadfence();
@@ -2244,7 +1508,7 @@ __global__ void __launch_bounds__(kThreads) k_record(const __grid_constant__ Act
   __threadfence();
   if (threadIdx.x == 0) *p.ticket = 0;  // the next launch follows in stream order
   const int kind = scan_sh.kind;
-  if (threadIdx.x < 32) relay_reduce(p, kind, rec.seq);
+  if (threadIdx.x < 32) reduce_answers(p, kind, rec.seq);
 }
 
 }  // namespace kai

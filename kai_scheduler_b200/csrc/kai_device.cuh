@@ -5,10 +5,12 @@
 //   queue tables  resource-major f64 [3][Q]
 //   task request  task-major f64 [T][R]
 //   session state (one copy): task status/node/virtual, queue allocated, node idle/releasing
-//   replica state (one copy per CTA of the persistent action kernel): the mutable part of the
-//     session that the replicated sequencer (thread 0 of every CTA) updates in lock step
+//
+// It also holds the few helpers that the kernels and the host sequencer both run (__host__ __device__): the f64
+// wrappers, the job key, the tile row striping, the tracker events and the node-delta arithmetic.
 #pragma once
 #include <cstdint>
+#include <cstring>
 #include <cuda_runtime.h>
 
 #include "../../include/kai_engine.h"
@@ -16,13 +18,13 @@
 namespace kai {
 
 constexpr int QR = KAI_QRES;
-constexpr int kThreads = 128;          // threads per CTA of the action kernel (4 warps: cheap barriers/reductions)
+constexpr int kThreads = 128;          // threads per scanner CTA of k_record (4 warps: cheap barriers/reductions)
 constexpr int kMaxGrid = 1024;         // exchange slots per GPU
 constexpr uint32_t kNoRank = 0xFFFFFFFFu;
 constexpr int kDecWords = 16;         // tagged words of one decision record
 constexpr int kMaxDelta = 256;        // node deltas carried by one decision record
-constexpr int kTopM = 4;              // candidates every scanner returns per sweep (host-sequenced mode)
-constexpr int kListScanners = 2048;   // scanners of all GPUs of a box (list lines in host memory)
+constexpr int kTopM = 4;              // candidates every scanner returns per list sweep
+constexpr int kListScanners = 2048;   // scanner lines per parity of d_list
 constexpr int kListLineWords = 8;     // one 64-byte line = 4 tagged words
 constexpr int kListLines = 1 + kTopM; // line 0: the M candidate words, lines 1..M: row values of candidate m
 constexpr int kMaxDomLevels = 8;      // topology levels of all Topology CRs together (rows keep one domain id per level)
@@ -34,6 +36,139 @@ constexpr int kActiveAllocated =
     KAI_POD_ALLOCATED | KAI_POD_PIPELINED | KAI_POD_BINDING | KAI_POD_BOUND | KAI_POD_RUNNING;
 constexpr int kAlive = kActiveAllocated | KAI_POD_PENDING | KAI_POD_GATED;
 constexpr int kAllocatedStatuses = KAI_POD_ALLOCATED | KAI_POD_BOUND | KAI_POD_BINDING | KAI_POD_RUNNING;
+
+// ---------------------------------------------------------------------------------------------
+// shared by the kernels and the host sequencer
+// ---------------------------------------------------------------------------------------------
+#define KAI_HD __host__ __device__
+
+// IEEE binary64 without contraction on both sides
+KAI_HD inline double kadd(double a, double b) {
+#ifdef __CUDA_ARCH__
+  return __dadd_rn(a, b);
+#else
+  return a + b;  // host translation unit is built with -ffp-contract=off
+#endif
+}
+KAI_HD inline double ksub(double a, double b) {
+#ifdef __CUDA_ARCH__
+  return __dsub_rn(a, b);
+#else
+  return a - b;
+#endif
+}
+KAI_HD inline double kmul(double a, double b) {
+#ifdef __CUDA_ARCH__
+  return __dmul_rn(a, b);
+#else
+  return a * b;
+#endif
+}
+KAI_HD inline double kdiv(double a, double b) {
+#ifdef __CUDA_ARCH__
+  return __ddiv_rn(a, b);
+#else
+  return a / b;
+#endif
+}
+KAI_HD inline unsigned long long kbits(double x) {
+  unsigned long long u;
+  memcpy(&u, &x, 8);
+  return u;
+}
+KAI_HD inline double requestable_share(double max_allowed, double request) {
+  if (max_allowed == KAI_UNLIMITED) return request;
+  return fmin(max_allowed, request);
+}
+// resource_share.go:51-61
+KAI_HD inline double allocatable_share(double deserved, double fair, double max_allowed) {
+  if (deserved == KAI_UNLIMITED) return max_allowed;
+  double a = fmax(deserved, fair);
+  if (max_allowed != KAI_UNLIMITED) a = fmin(max_allowed, a);
+  return a;
+}
+
+KAI_HD inline unsigned long long make_job_key(int priority, int cls, int order_rank) {
+  unsigned long long pinv = (unsigned long long)(unsigned int)(0x40000000 - priority) & 0x7fffffffull;
+  return (pinv << 33) | ((unsigned long long)cls << 31) | (unsigned long long)(order_rank & 0x7fffffff);
+}
+
+struct Track {  // global min/max of NonAllocated(res) over nodes with Allocatable(res) != 0 (pack.go:66-86)
+  double mn, mx;
+  int cnt_mn, cnt_mx;
+  int dirty;
+};
+// tracker event bits per resource (gpu bits 0-2, cpu bits 3-5)
+enum { WF_B_EQ_MX = 1, WF_A_EQ_MN = 2, WF_A_LT_MN = 4 };
+KAI_HD inline uint32_t track_flags(const Track &t, double b, double a) {
+  uint32_t f = 0;
+  if (b == t.mx) f |= WF_B_EQ_MX;
+  if (a < t.mn)
+    f |= WF_A_LT_MN;
+  else if (a == t.mn)
+    f |= WF_A_EQ_MN;
+  return f;
+}
+
+constexpr uint32_t kTileDom = 1u << 29;  // tile flag bits 29, 28, 27, 26: row belongs to the domain selected in slot 0..3
+constexpr int kDomSlots = 4;             // nesting depth of SubGroupSet / PodSet constraints the scanners can intersect
+// XB_RESTRICT_DOM sweeps carry the number of active slots in xbits bits 8..10: a row must sit in all of them
+KAI_HD inline uint32_t dom_need_mask(unsigned int xbits) {
+  const unsigned int n = (xbits >> 8) & 7u;
+  uint32_t m = 0;
+  for (unsigned int i = 0; i < n && i < (unsigned int)kDomSlots; i++) m |= kTileDom >> i;
+  return m;
+}
+
+struct Tile {  // node tile of one scanner CTA
+  double *I, *L;        // [R][npc]
+  double *Agpu, *Acpu;  // [npc]
+  double *gpu_count;    // [npc]
+  int *rank;            // [npc]
+  uint32_t *flags;      // [npc]
+  int *node;            // [npc] node index of the row
+  int *dom;             // [n_dom_levels][npc] topology domain per level
+  int n_dom_levels;
+  int npc, count, R;
+  // Rows are striped by NAME RANK over the GPUs of the box and over the scanners of a GPU: row j of scanner `my`
+  // of shard `shard` is the node of name rank (j * nscan + my) * nshard + shard.  Consecutive ranks land on
+  // different scanners, so the global top-K rows of a sweep come from ~K different scanners.
+  int nscan, my, nshard, shard;
+  int nscan_log2;  // log2(nscan) when nscan is a power of two, else -1
+};
+KAI_HD inline int tile_row_rank(const Tile &tl, int ln) { return (ln * tl.nscan + tl.my) * tl.nshard + tl.shard; }
+KAI_HD inline bool tile_owns(const Tile &tl, unsigned int rank, int &ln) {
+  unsigned int q = rank;
+  if (tl.nshard != 1) {  // one GPU: every rank is this shard's
+    q = rank / (unsigned int)tl.nshard;
+    if (rank - q * (unsigned int)tl.nshard != (unsigned int)tl.shard) return false;
+  }
+  unsigned int j;
+  if (tl.nscan_log2 >= 0) {  // scanner count is a power of two (256 by default): no integer division on the device
+    j = q >> tl.nscan_log2;
+    if ((q & ((1u << tl.nscan_log2) - 1u)) != (unsigned int)tl.my) return false;
+  } else {
+    j = q / (unsigned int)tl.nscan;
+    if (q - j * (unsigned int)tl.nscan != (unsigned int)tl.my) return false;
+  }
+  ln = (int)j;
+  return true;
+}
+
+// ---- node mutations (node_info.go:457-551) are queued as deltas for the scanner that owns the node ----
+enum { ND_ADD = 0, ND_ADD_PIPELINED = 1, ND_ADD_RELEASING = 2, ND_REM = 3, ND_REM_PIPELINED = 4, ND_REM_RELEASING = 5,
+       ND_FEAS_SET = 6, ND_FEAS_CLR = 7 };  // 6, 7: feasible-set membership of the row (no task attached)
+// applied by the owning scanner to its tile row (lane r handles resource r) and by the host to its node mirror
+KAI_HD inline void apply_delta_row(double &I, double &L, int code, double v) {
+  switch (code) {
+    case ND_ADD: I = ksub(I, v); break;
+    case ND_ADD_PIPELINED: L = ksub(L, v); break;
+    case ND_ADD_RELEASING: L = kadd(L, v); I = ksub(I, v); break;
+    case ND_REM: I = kadd(I, v); break;
+    case ND_REM_PIPELINED: L = kadd(L, v); break;
+    case ND_REM_RELEASING: L = ksub(L, v); I = kadd(I, v); break;
+  }
+}
 
 struct Op {  // framework/statement.go operations (allocate / pipeline / evict / undo)
   int kind, task, prev_status, prev_node, next_node, prev_virtual, undo_index, pad;
@@ -111,7 +246,6 @@ struct DevSnap {
   Op *ops;                     // [ops_cap] statement log
   int *tta;                    // [max_job_tasks + 1]
   int *ps_order;               // [max_job_podsets + 1]
-  unsigned char *hot_global;   // hot arrays when they do not fit in shared memory
   JobRec *jrec;                // [J]
 };
 
@@ -125,9 +259,8 @@ struct QKey {
   unsigned char over, starved, viol, valid;
 };
 
-// Mutable state the sequencer CTA works on.  The "hot" per-queue arrays live in its shared memory when
-// they fit (ActionParams.hot_in_smem), otherwise in global memory; the cold arrays are the session
-// arrays in HBM/L2 themselves (single copy).
+// Mutable state the host sequencer works on.  The "hot" per-queue arrays are its own copy; the cold arrays are the
+// session arrays of the host mirror themselves (single copy).
 struct Replica {
   // hot: per queue
   double *q_alloc, *q_alloc_np;  // [3][Q]
@@ -152,36 +285,23 @@ struct Replica {
   int *ps_order;              // [max_job_podsets]
 };
 
+// Parameters of k_record and k_merge_cluster for one action.
 struct ActionParams {
   DevSnap s;
   kai_config cfg;
-  int action;
-  int grid;             // CTAs of this GPU
-  int nodes_per_cta;    // node rows per CTA (tile height)
-  int ops_cap;
-  unsigned long long *dbuf;  // decision record: [2][kDecWords] tagged 128-bit words (sequencer -> scanners)
-  unsigned long long *delta; // node delta list: [2][kMaxDelta] tagged words {name_rank(node) | code<<28 | task<<32, seq}
+  int scanners;              // CTAs of k_record
+  int nodes_per_cta;         // node rows per scanner (tile height)
   unsigned long long *xbuf;  // exchange slots: [2][kMaxGrid][8] u64 (tagged 128-bit words A, B, C, D)
   unsigned long long *mmbuf; // min/max exchange: [2][kMaxGrid][8] u64
-  kai_job_visit *visits;     // [visits_cap]
-  int visits_cap;
-  long long *counters;  // [16]: n_visits, sweeps, nodes_scanned, pods_placed, pods_evicted, minmax_exchanges, error, seq, phase timers
-  unsigned int seq0;    // first exchange sequence number of this launch
-  int hot_in_smem;      // hot replica arrays carved from dynamic shared memory after the node tile
-  size_t tile_bytes, hot_bytes;
-  int batching;         // same-node batching of consecutive identical pods (1 = on)
-  int mode;             // 0 = device-resident sequencer (CTA 0), 1 = host-sequenced (CTA 0 relays host records)
-  unsigned long long *h_rec, *h_delta;  // mode 1: decision record / delta words in pinned mapped host memory
-  unsigned long long *h_slot, *h_mmslot;  // mode 1: this GPU's reduced answer line [2][kSlotWords] in (shared) host memory
-  int spin_log2;        // watchdog: polls before a wait is declared dead
-  int topm;             // mode 1: scanners answer with their kTopM best rows (0 = single best through the relay)
-  unsigned long long *h_list;  // mode 1: [2][kListScanners][kListLines][kListLineWords] in (shared) host memory
-  int scanner_base;     // global index of this GPU's scanner 0 in h_list
-  const int *node_domain;  // [n_dom_levels][N] topology domain of every node per level (-1 = label missing), or null
+  long long *counters;       // [48]: watchdog (24..27) and KAI_PROFILE cycle counts
+  unsigned long long *h_slot, *h_mmslot;  // this GPU's reduced answer line [2][kSlotWords] in (shared) host memory
+  int spin_log2;             // watchdog: polls before a wait is declared dead
+  int topm;                  // scanners answer with their kTopM best rows (0 = single best through the last CTA)
+  unsigned long long *d_list;  // [2][kListScanners][kListLines][kListLineWords]: the scanners' top-M lines
+  const int *node_domain;    // [n_dom_levels][N] topology domain of every node per level (-1 = label missing), or null
   int n_dom_levels;
-  // ---- launch transport (mode 2): one kernel launch per decision record, node tiles resident in global memory ----
-  unsigned char *g_tiles;      // [scanners][g_tile_stride] tiles in the layout of the shared-memory tile
-  size_t g_tile_stride;
+  unsigned char *g_tiles;      // [scanners][g_tile_stride] tiles in the layout of tile_carve
+  size_t g_tile_stride, tile_bytes;
   unsigned char *g_scan_state; // [scanners][kScanStateBytes]: preferred level + per-domain score buckets of each scanner
   unsigned int *ticket;        // CTAs that finished the current launch (the last one reduces the answers)
   double *mm_result;           // [4] gpu mn, gpu mx, cpu mn, cpu mx of the last MINMAX launch (read by XB_FUSED_MM sweeps)
@@ -189,14 +309,14 @@ struct ActionParams {
   int fused_in_kernel;         // XB_FUSED_MM sweeps exchange their extremes inside the launch (cooperative launch: all CTAs resident)
 };
 
-constexpr int kMergeCap = 1024;                      // candidates k_merge sorts, one per thread (scanners x kTopM)
+constexpr int kMergeCap = 1024;                      // candidates k_merge_cluster sorts, one per thread (scanners x kTopM)
 constexpr int kCEntryWords = 6;                      // score, meta, Ig, Lg, Ic, Lc
 constexpr int kCListWords = 2 + kMergeCap * kCEntryWords;  // header {count | more << 31, tag} + entries
 constexpr int kScanStateBytes = 16 + kDomBuckets;
 constexpr int kMaxDeltaL = kMaxDelta;
-enum { DK_LOAD = 6 };  // launch transport: load the tiles from the session tables (first launch of an action)
+enum { DK_LOAD = 6 };  // load the tiles from the session tables (first launch of an action)
 
-// One decision record of the launch transport, passed by value in the kernel parameter space.
+// One decision record, passed to k_record by value in the kernel parameter space.
 struct LaunchRec {
   unsigned long long dw[kDecWords];
   unsigned int seq;

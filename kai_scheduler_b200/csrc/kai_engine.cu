@@ -4,8 +4,8 @@
 // children CSR, jobs grouped by leaf queue in JobOrderFn order, tasks per podset in TaskOrderFn
 // order, name-rank inverse), stages everything through one pinned buffer into HBM (or, for a resident
 // snapshot, refreshes the per-cycle columns only), runs the open-session kernels, drives the sweep
-// kernels of an action from the host sequencer (one k_record launch per decision record; or the
-// persistent k_action kernel), and copies results back.
+// kernels of an action from the host sequencer (one k_record launch per decision record), and copies
+// results back.
 //
 // There is NO CPU fallback: without a usable CUDA device kai_engine_create fails.
 #include <algorithm>
@@ -90,10 +90,8 @@ struct Staging {  // pinned host staging buffer mirrored 1:1 onto a device arena
 size_t align_up(size_t v, size_t a) { return (v + a - 1) & ~(a - 1); }
 
 constexpr int kShmRanks = 16;  // GPUs of one box that can share the exchange segment
-// layout of the shared exchange segment (u64 words): answer lines | min/max lines | top-M lines | merged lists per rank
-size_t shm_clist_offset_words() {
-  return (size_t)2 * 2 * kMaxGrid * kSlotWords + (size_t)2 * kListScanners * kListLines * kListLineWords;
-}
+// layout of the shared exchange segment (u64 words): answer lines | min/max lines | merged lists per rank
+size_t shm_clist_offset_words() { return (size_t)2 * 2 * kMaxGrid * kSlotWords; }
 
 }  // namespace
 
@@ -114,28 +112,23 @@ struct kai_engine {
   DeviceArena dmisc;     // exchange buffers, counters, visits, fair-share scratch
   DevSnap ds;
   int R = 4, N = 0, Q = 0, J = 0, S = 0, T = 0;
-  int grid = 0, npc = 0;
-  size_t smem_bytes = 0, replica_bytes = 0, tile_bytes = 0, hot_bytes = 0;
-  bool hot_in_smem = false;
+  size_t hot_bytes = 0;  // the host sequencer's per-queue arrays
   int ops_cap = 0, visits_cap = 0;
-  unsigned long long *xbuf = nullptr, *mmbuf = nullptr, *dbuf = nullptr;
-  unsigned long long *delta = nullptr;
-  // host-sequenced mode
-  unsigned long long *h_pinned = nullptr;  // one pinned mapped allocation: rec | delta | slots | mm
-  unsigned long long *h_rec = nullptr, *h_delta = nullptr, *h_slots = nullptr, *h_mm = nullptr, *h_list = nullptr;
+  unsigned long long *xbuf = nullptr, *mmbuf = nullptr;
+  unsigned long long *h_pinned = nullptr;  // one pinned mapped allocation: delta | slots | mm
+  unsigned long long *h_delta = nullptr, *h_slots = nullptr, *h_mm = nullptr;
   HostBackend hb;
-  // launch transport (default): one k_record launch per decision record, node tiles resident in global memory
+  // one k_record launch per decision record, node tiles resident in global memory
   DeviceArena dlaunch;
   int lgrid = 0, lnpc = 0;  // scanners (= CTAs of k_record) and rows per scanner
-  size_t ltile_stride = 0, ltile_bytes = 0, lsmem_bytes = 0;
+  size_t ltile_stride = 0, ltile_bytes = 0;  // ltile_bytes: also the dynamic shared memory of k_record (staged tile)
   unsigned char *g_tiles = nullptr, *g_scan_state = nullptr;
   unsigned long long *d_list = nullptr;
   unsigned int *ticket = nullptr;
   double *mm_result = nullptr;
   unsigned long long *h_clist = nullptr;  // pinned mapped: [2][kCListWords]
-  ActionParams lp;                        // parameters of the running action (launch transport)
+  ActionParams lp;                        // parameters of the running action
   long long record_launches = 0;
-  bool merge_cluster = true;  // k_merge_cluster (4-CTA cluster) instead of the one-CTA k_merge (KAI_MERGE=single)
   // multi-GPU (one engine per process per GPU): the reduced answer lines of all GPUs live in one POSIX shm
   // segment that every process maps and registers with CUDA; each host sequencer reads all lines.
   unsigned long long *shm_base = nullptr;  // [slots | mm], each [2][kMaxGrid][kSlotWords]
@@ -151,11 +144,11 @@ struct kai_engine {
   std::vector<std::array<int, 3>> on_extra;  // (task, node, status) node entries beyond two per task (kai_solver.cuh)
   SolverScratch solver_scratch;              // the solver's per-node / per-job / per-task scratch (sized at first use)
   std::vector<double> h_mirror;  // host mirror of Idle / Releasing, node-major [N][2][R]
-  std::vector<double> h_tmp;     // staging for the re-read after a device-sequenced action
+  std::vector<double> h_tmp;     // staging for the re-read of the node tables when the mirror is stale
   int *d_node_domain = nullptr;
   TopologyHost topo;
   int n_dom_levels = 0;
-  bool mirror_valid = false;  // h_ig / h_lg followed every delta since the load (host-sequenced actions only)
+  bool mirror_valid = false;  // h_mirror followed every delta since the load
   std::vector<int> job_signature;
   std::vector<double> q_preempt_mrt, q_reclaim_mrt, j_last_start;  // plugins/minruntime inputs (host only)
   std::vector<double> j_stale_since;                               // stalegangeviction input (host only)
@@ -286,16 +279,13 @@ static int reset_sequence_if_due(kai_engine *e) {
   }
   if (e->seq <= at || e->cfg.shard_count != 1) return KAI_OK;
   e->seq = 2;
-  memset(e->h_pinned, 0, ((size_t)2 * kDecWords * 2 + (size_t)2 * kMaxDelta * 2 + (size_t)2 * 2 * kMaxGrid * kSlotWords +
-                          (size_t)2 * kListScanners * kListLines * kListLineWords) * 8);
+  memset(e->h_pinned, 0, ((size_t)2 * kMaxDelta * 2 + (size_t)2 * 2 * kMaxGrid * kSlotWords) * 8);
   memset(e->h_clist, 0, (size_t)2 * kCListWords * 8);
   const size_t list_words = (size_t)2 * kListScanners * kListLines * kListLineWords, xb = (size_t)2 * kMaxGrid * 8 * 8;
   if (e->d_list) CK(cudaMemsetAsync(e->d_list, 0, list_words * 8, e->stream));
   if (e->mm_result) CK(cudaMemsetAsync(e->mm_result, 0, 32, e->stream));
   if (e->xbuf) CK(cudaMemsetAsync(e->xbuf, 0, xb, e->stream));
   if (e->mmbuf) CK(cudaMemsetAsync(e->mmbuf, 0, xb, e->stream));
-  if (e->dbuf) CK(cudaMemsetAsync(e->dbuf, 0, sizeof(unsigned long long) * 2 * kDecWords * 2, e->stream));
-  if (e->delta) CK(cudaMemsetAsync(e->delta, 0, sizeof(unsigned long long) * 2 * kMaxDelta * 2, e->stream));
   return KAI_OK;
 }
 
@@ -411,19 +401,16 @@ int kai_engine_create(const kai_config *cfg, kai_engine **out) {
   }
   for (auto &ev : e->ev) cudaEventCreate(&ev);
   cudaEventCreateWithFlags(&e->ev_mirror, cudaEventDisableTiming);
-  {  // pinned, device-mapped protocol buffers of the host-sequenced mode
-    const size_t list_words = (size_t)2 * kListScanners * kListLines * kListLineWords;
-    size_t words = (size_t)2 * kDecWords * 2 + (size_t)2 * kMaxDelta * 2 + (size_t)2 * 2 * kMaxGrid * kSlotWords + list_words;
+  {  // pinned, device-mapped buffers of the host sequencer
+    size_t words = (size_t)2 * kMaxDelta * 2 + (size_t)2 * 2 * kMaxGrid * kSlotWords;
     if (cudaHostAlloc((void **)&e->h_pinned, words * 8, cudaHostAllocMapped | cudaHostAllocPortable) != cudaSuccess) {
       delete e;
       return KAI_ERR_CUDA;
     }
     memset(e->h_pinned, 0, words * 8);
-    e->h_rec = e->h_pinned;
-    e->h_delta = e->h_rec + (size_t)2 * kDecWords * 2;
+    e->h_delta = e->h_pinned;
     e->h_slots = e->h_delta + (size_t)2 * kMaxDelta * 2;
     e->h_mm = e->h_slots + (size_t)2 * kMaxGrid * kSlotWords;
-    e->h_list = e->h_mm + (size_t)2 * kMaxGrid * kSlotWords;
     if (cudaHostAlloc((void **)&e->h_clist, (size_t)2 * kCListWords * 8, cudaHostAllocMapped | cudaHostAllocPortable) != cudaSuccess) {
       delete e;
       return KAI_ERR_CUDA;
@@ -745,11 +732,10 @@ int kai_engine_load_snapshot(kai_engine *e, const kai_snapshot *s) {
   size_t o_ops = reserve_up(sizeof(Op) * (size_t)ops_cap);
   size_t o_tta = reserve_up((size_t)(max_job_tasks + 1) * 4), o_psord = reserve_up((size_t)(max_job_podsets + 1) * 4);
   auto a16 = [](size_t b) { return (b + 15) & ~(size_t)15; };
-  // hot per-queue sequencer arrays — must match the carving in sequencer_main
+  // hot per-queue arrays of the host sequencer — must match the carving in kai_engine_run
   const size_t hot = 2 * a16(sizeof(double) * QR * Q) + a16(sizeof(QKey) * (size_t)Q) + 5 * a16(sizeof(int) * (size_t)Q) +
                      a16(sizeof(int) * (size_t)(top.size() + 1)) + a16((size_t)Q) +
                      a16(sizeof(unsigned int) * (size_t)((J + 31) / 32 + 1));
-  size_t o_hot = reserve_up(hot + 16);
   size_t o_jrec = reserve_up(sizeof(JobRec) * (size_t)std::max(J, 1));
   const size_t zero_begin = o_tvirt, zero_bytes = up - o_tvirt;
 
@@ -902,7 +888,6 @@ int kai_engine_load_snapshot(kai_engine *e, const kai_snapshot *s) {
   ds.ops = (Op *)(d + o_ops);
   ds.tta = (int *)(d + o_tta);
   ds.ps_order = (int *)(d + o_psord);
-  ds.hot_global = d + o_hot;
   ds.jrec = (JobRec *)(d + o_jrec);
   {  // host view: every pointer of ds rebased onto the staging buffer (same offsets)
     static_assert(sizeof(void *) == 8, "64-bit only");
@@ -924,25 +909,11 @@ int kai_engine_load_snapshot(kai_engine *e, const kai_snapshot *s) {
     rb(h_.t_req); rb(h_.t_job); rb(h_.t_podset); rb(h_.osum); rb(h_.t_nominated); rb(h_.t_pred_class); rb(h_.t_status);
     rb(h_.t_node); rb(h_.t_node_status); rb(h_.t_virtual); rb(h_.pred_mask); rb(h_.total); rb(h_.q_allocatable);
     rb(h_.j_key0); rb(h_.leaf_sorted); rb(h_.leaf_count); rb(h_.ps_cnt0); rb(h_.j_req); rb(h_.j_req_valid);
-    rb(h_.ops); rb(h_.tta); rb(h_.ps_order); rb(h_.hot_global); rb(h_.jrec);
+    rb(h_.ops); rb(h_.tta); rb(h_.ps_order); rb(h_.jrec);
   }
 
-  // ---------------- launch geometry of the action kernel ----------------
-  // CTA 0 = sequencer, CTAs 1..grid-1 = scanners that split the node rows
-  int grid = std::min(e->num_sms, kMaxGrid);
-  if (const char *g = getenv("KAI_GRID")) {
-    int v = atoi(g);
-    if (v >= 2) grid = std::min(v, grid);
-  }
+  // ---------------- launch geometry of k_record ----------------
   const int n_shard_rows = (N + e->cfg.shard_count - 1) / e->cfg.shard_count;  // rows of the largest shard
-  if (N > 0) grid = std::min(grid, n_shard_rows + 1);  // at least one node per scanner when possible
-  grid = std::max(grid, 2);
-  if (const char *g = getenv("KAI_GRID_EXACT")) {  // tests: force scanners without nodes as well
-    int v = atoi(g);
-    if (v >= 2) grid = std::min(std::min(v, e->num_sms), kMaxGrid);
-  }
-  int npc = std::max(1, (n_shard_rows + (grid - 1) - 1) / (grid - 1));
-  npc = (npc + 1) & ~1;  // keep the int arrays 8-byte aligned
   const int n_dom_levels = (s->n_topologies > 0 && s->topology_level_begin && s->node_domain) ? s->topology_level_begin[s->n_topologies] : 0;
   if (n_dom_levels > kMaxDomLevels) return e->fail(KAI_ERR_UNSUPPORTED, "more topology levels than kMaxDomLevels");
   // a GPU request with a fractional part is a shared-GPU pod (gpu_resource_requirment.go:52-54,230-234): it needs the
@@ -952,21 +923,10 @@ int kai_engine_load_snapshot(kai_engine *e, const kai_snapshot *s) {
     const double g = s->task_req[(size_t)t * R + KAI_RES_GPU];
     if (g != (double)(long long)g) return e->fail(KAI_ERR_UNSUPPORTED, "fractional GPU request: GPU sharing is outside this engine's scope");
   }
-  size_t tile_bytes = align_up((size_t)npc * ((size_t)2 * R * 8 + 3 * 8 + 4 + 4 + 4 + (size_t)4 * n_dom_levels), 16);
-  const size_t smem_limit = (size_t)e->max_smem_optin - 28 * 1024;  // static shared memory of k_action
-  if (tile_bytes > smem_limit)
-    return e->fail(KAI_ERR_UNSUPPORTED, "node tile does not fit in shared memory (N too large for one GPU tile)");
-  bool hot_in_smem = hot <= smem_limit;
-  if (getenv("KAI_NO_SMEM_HOT")) hot_in_smem = false;
-  e->grid = grid;
-  e->npc = npc;
-  e->tile_bytes = tile_bytes;
   e->hot_bytes = hot;
-  e->hot_in_smem = hot_in_smem;
-  e->smem_bytes = std::max(tile_bytes, hot_in_smem ? hot : (size_t)0);
   e->ops_cap = ops_cap;
   e->visits_cap = std::max(16, 2 * J + T + 16);
-  {  // launch transport: scanners = CTAs of k_record; k_merge sorts scanners x kTopM candidates (<= kMergeThreads)
+  {  // scanners = CTAs of k_record; k_merge_cluster sorts scanners x kTopM candidates (<= kMergeThreads)
     int lg = 1;
     while (lg * 2 <= std::min(2 * e->num_sms, kMergeThreads / kTopM)) lg *= 2;  // 256 on H100 (132 SMs): a power of two keeps the merge sort full
     if (const char *g = getenv("KAI_LAUNCH_GRID")) {
@@ -974,18 +934,20 @@ int kai_engine_load_snapshot(kai_engine *e, const kai_snapshot *s) {
       if (v >= 1) lg = std::min(v, kMergeThreads / kTopM);
     }
     if (N > 0) lg = std::min(lg, std::max(1, n_shard_rows));
-    if (const char *g = getenv("KAI_GRID_EXACT")) {  // tests: the same forced geometries as the persistent kernel (grid - 1 scanners)
+    if (const char *g = getenv("KAI_GRID_EXACT")) {  // tests: force v - 1 scanners, including scanners without nodes
       int v = atoi(g);
       if (v >= 2) lg = std::min(v - 1, kMergeThreads / kTopM);
     }
     int lnpc = std::max(1, (n_shard_rows + lg - 1) / lg);
-    lnpc = (lnpc + 1) & ~1;
+    lnpc = (lnpc + 1) & ~1;  // keep the int arrays 8-byte aligned
+    const size_t ltile_bytes = align_up((size_t)lnpc * ((size_t)2 * R * 8 + 3 * 8 + 4 + 4 + 4 + (size_t)4 * n_dom_levels), 16);
+    // a sweep stages the scanner's tile in dynamic shared memory, next to k_record's static shared memory
+    if (ltile_bytes > (size_t)e->max_smem_optin - 40 * 1024)
+      return e->fail(KAI_ERR_UNSUPPORTED, "node tile does not fit in shared memory (N too large for one GPU tile)");
     e->lgrid = lg;
     e->lnpc = lnpc;
-    e->ltile_bytes = align_up((size_t)lnpc * ((size_t)2 * R * 8 + 3 * 8 + 4 + 4 + 4 + (size_t)4 * n_dom_levels), 16);
-    e->ltile_stride = align_up(e->ltile_bytes, 256);
-    // dynamic shared memory of k_record: the staged tile during a sweep (scanned from global memory when it does not fit)
-    e->lsmem_bytes = e->ltile_bytes <= (size_t)e->max_smem_optin - 40 * 1024 ? e->ltile_bytes : 16;
+    e->ltile_bytes = ltile_bytes;
+    e->ltile_stride = align_up(ltile_bytes, 256);
     const size_t list_words = (size_t)2 * kListScanners * kListLines * kListLineWords;
     CK(e->dlaunch.reserve((size_t)lg * e->ltile_stride + (size_t)lg * align_up(kScanStateBytes, 256) + list_words * 8 + 4096));
     e->g_tiles = e->dlaunch.take<unsigned char>((size_t)lg * e->ltile_stride);
@@ -999,8 +961,7 @@ int kai_engine_load_snapshot(kai_engine *e, const kai_snapshot *s) {
   }
   {
     size_t xb = (size_t)2 * kMaxGrid * 8 * 8;
-    size_t misc = 2 * xb + 256 + sizeof(long long) * 48 + sizeof(kai_job_visit) * (size_t)e->visits_cap + 2 * QN * 8 + 4096 +
-                  sizeof(unsigned long long) * 2 * kDecWords * 2 + sizeof(unsigned long long) * 2 * kMaxDelta * 2 + 1024;
+    size_t misc = 2 * xb + 256 + sizeof(long long) * 48 + sizeof(kai_job_visit) * (size_t)e->visits_cap + 2 * QN * 8 + 4096;
     CK(e->dmisc.reserve(misc));
     e->xbuf = e->dmisc.take<unsigned long long>(2 * kMaxGrid * 8);
     e->mmbuf = e->dmisc.take<unsigned long long>(2 * kMaxGrid * 8);
@@ -1008,10 +969,6 @@ int kai_engine_load_snapshot(kai_engine *e, const kai_snapshot *s) {
     e->d_visits = e->dmisc.take<kai_job_visit>(e->visits_cap);
     e->fs_w = e->dmisc.take<double>(QN + 1);
     e->fs_rr = e->dmisc.take<double>(QN + 1);
-    e->dbuf = e->dmisc.take<unsigned long long>(2 * kDecWords * 2);
-    e->delta = e->dmisc.take<unsigned long long>(2 * kMaxDelta * 2);
-    CK(cudaMemsetAsync(e->delta, 0, sizeof(unsigned long long) * 2 * kMaxDelta * 2, e->stream));
-    CK(cudaMemsetAsync(e->dbuf, 0, sizeof(unsigned long long) * 2 * kDecWords * 2, e->stream));
     CK(cudaMemsetAsync(e->xbuf, 0, xb, e->stream));
     CK(cudaMemsetAsync(e->mmbuf, 0, xb, e->stream));
   }
@@ -1077,12 +1034,12 @@ int kai_engine_fair_share(kai_engine *e, kai_result *out) {
   return download(e, out, 0, 0, 0);
 }
 
-// Launch transport: enqueue the kernel launch(es) of one decision record on the engine's stream.
+// Enqueue the kernel launch(es) of one decision record on the engine's stream.
 static bool engine_launch_record(void *ctx, const LaunchRec &rec) {
   kai_engine *e = (kai_engine *)ctx;
   const int kind = (int)(rec.dw[0] & 0xff);
   const unsigned int xbits = (unsigned int)((rec.dw[0] >> 48) & 0xffff);
-  const size_t dyn = e->lsmem_bytes;
+  const size_t dyn = e->ltile_bytes;
   if (kind == DK_SCAN && (xbits & XB_FUSED_MM) && e->lp.fused_in_kernel) {
     // every CTA is resident (checked at load): the scanners exchange their binpack extremes among themselves
     // through tagged device slots inside this one launch
@@ -1104,10 +1061,7 @@ static bool engine_launch_record(void *ctx, const LaunchRec &rec) {
     k_record<<<e->lgrid, kThreads, dyn, e->stream>>>(e->lp, rec);
     e->record_launches++;
     if (kind == DK_TOPK || (kind == DK_SCAN && e->lp.topm && !(xbits & XB_SINGLE))) {  // list answer: sort, cut, stream to the host
-      if (e->merge_cluster)
-        k_merge_cluster<<<kMergeCtas, kMergeCtaThreads, kMergeCtaSmemBytes, e->stream>>>(e->lp, rec.seq, kind == DK_SCAN ? 1 : 0);
-      else
-        k_merge<<<1, kMergeThreads, kMergeSmemBytes, e->stream>>>(e->lp, rec.seq, kind == DK_SCAN ? 1 : 0);
+      k_merge_cluster<<<kMergeCtas, kMergeCtaThreads, kMergeCtaSmemBytes, e->stream>>>(e->lp, rec.seq, kind == DK_SCAN ? 1 : 0);
       e->record_launches++;
     }
   }
@@ -1127,448 +1081,366 @@ int kai_engine_run(kai_engine *e, kai_action action, kai_result *out) {
   memset(&p, 0, sizeof(p));
   p.s = e->ds;
   p.cfg = e->cfg;
-  p.action = (int)action;
-  p.grid = e->grid;
-  p.nodes_per_cta = e->npc;
-  p.dbuf = e->dbuf;
-  p.delta = e->delta;
-  p.ops_cap = e->ops_cap;
   p.xbuf = e->xbuf;
   p.mmbuf = e->mmbuf;
-  p.visits = e->d_visits;
-  p.visits_cap = e->visits_cap;
   p.counters = e->counters;
   p.node_domain = e->d_node_domain;
   p.n_dom_levels = e->n_dom_levels;
-  p.seq0 = e->seq;
-  p.hot_in_smem = e->hot_in_smem ? 1 : 0;
-  p.tile_bytes = e->tile_bytes;
-  p.hot_bytes = e->hot_bytes;
-  p.batching = getenv("KAI_NO_BATCHING") ? 0 : 1;
-  CK(cudaFuncSetAttribute(k_action, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)e->smem_bytes));
-  int max_blocks = 0;
-  CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&max_blocks, k_action, kThreads, e->smem_bytes));
-  if (max_blocks < 1 || max_blocks * e->num_sms < e->grid)
-    return e->fail(KAI_ERR_CUDA, "action kernel cannot be made co-resident");
-  const char *mode_env = getenv("KAI_SEQUENCER");
-  const bool host_mode = !(mode_env && strcmp(mode_env, "device") == 0);
-  if (!host_mode && e->cfg.shard_count > 1) return e->fail(KAI_ERR_UNSUPPORTED, "device-resident sequencer is single-GPU");
-  if (solver_action && !host_mode) return e->fail(KAI_ERR_UNSUPPORTED, "reclaim / consolidation / preempt run host-sequenced");
-  if (solver_action && e->cfg.shard_count > 1 && !e->mirror_valid)
-    return e->fail(KAI_ERR_UNSUPPORTED, "multi-GPU solver actions need every earlier action of the cycle to be host-sequenced");
-  if (!host_mode) e->mirror_valid = false;
-  if (!host_mode && e->topo.any())
-    for (int j = 0; j < e->J; j++)
-      if (e->topo.constrained(j)) return e->fail(KAI_ERR_UNSUPPORTED, "topology constraints need the host-sequenced mode");
-  // transport of the host-sequenced mode: "launch" (default) = one k_record launch per decision record, tiles in global
-  // memory; "persistent" = the cooperative scan-server kernel polling records in pinned host memory
-  const char *tr_env = getenv("KAI_TRANSPORT");
-  const bool launch_mode = host_mode && !(tr_env && strcmp(tr_env, "persistent") == 0);
-  p.mode = host_mode ? (launch_mode ? 2 : 1) : 0;
-  p.spin_log2 = host_mode ? 26 : 22;
-  if (host_mode) {
-    p.h_rec = e->h_rec;
-    p.h_delta = e->h_delta;
-    // one reduced answer line per GPU; with several GPUs the lines live in the shared segment
-    unsigned long long *lines = e->cfg.shard_count > 1 ? e->shm_dev : e->h_slots;
-    unsigned long long *mm_lines = e->cfg.shard_count > 1 ? e->shm_dev + (size_t)2 * kMaxGrid * kSlotWords : e->h_mm;
-    p.h_slot = lines + (size_t)e->cfg.shard_rank * kSlotWords;
-    p.h_mmslot = mm_lines + (size_t)e->cfg.shard_rank * kSlotWords;
-    p.topm = (p.batching && !getenv("KAI_NO_TOPM")) ? 1 : 0;
-    p.h_list = e->cfg.shard_count > 1 ? e->shm_dev + (size_t)2 * 2 * kMaxGrid * kSlotWords : e->h_list;
-    p.scanner_base = e->cfg.shard_rank * (e->grid - 1);
-    if ((long long)e->cfg.shard_count * (e->grid - 1) > kListScanners) p.topm = 0;
-    if (launch_mode) {
-      if (e->cfg.shard_count > kShmRanks) return e->fail(KAI_ERR_UNSUPPORTED, "more GPUs than the exchange segment holds");
-      p.grid = e->lgrid + 1;  // scanners = grid - 1, as in the persistent kernel
-      p.nodes_per_cta = e->lnpc;
-      p.topm = (p.batching && !getenv("KAI_NO_TOPM")) ? 1 : 0;
-      p.h_list = e->d_list;  // the scanners' top-M lines stay on the device; the last CTA merges them
-      p.scanner_base = 0;
-      p.g_tiles = e->g_tiles;
-      p.g_tile_stride = e->ltile_stride;
-      p.g_scan_state = e->g_scan_state;
-      p.ticket = e->ticket;
-      p.mm_result = e->mm_result;
-      p.h_clist = e->cfg.shard_count > 1 ? e->shm_dev + shm_clist_offset_words() + (size_t)e->cfg.shard_rank * 2 * kCListWords : e->h_clist;
-      p.spin_log2 = 22;
-      p.tile_bytes = e->ltile_bytes;
-      p.hot_in_smem = e->ltile_bytes <= e->lsmem_bytes ? 1 : 0;  // the scanners stage their tile in shared memory for a sweep
-      {
-        int per_sm = 0;
-        CK(cudaFuncSetAttribute(k_record, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)e->lsmem_bytes));
-        CK(cudaFuncSetAttribute(k_merge, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMergeSmemBytes));
-        {
-          const char *mk = getenv("KAI_MERGE");
-          e->merge_cluster = !(mk && strcmp(mk, "single") == 0);
-        }
-        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_record, kThreads, e->lsmem_bytes));
-        p.fused_in_kernel = (per_sm * e->num_sms >= e->lgrid && !getenv("KAI_NO_FUSED_LAUNCH")) ? 1 : 0;
-      }
-    }
+  {  // values of modes the engine no longer has: refuse them, so that a run set up for one cannot report it
+    const char *tr = getenv("KAI_TRANSPORT"), *sq = getenv("KAI_SEQUENCER");
+    if (tr && strcmp(tr, "persistent") == 0)
+      return e->fail(KAI_ERR_UNSUPPORTED, "KAI_TRANSPORT=persistent is not supported: every decision record is one k_record launch");
+    if (sq && strcmp(sq, "device") == 0)
+      return e->fail(KAI_ERR_UNSUPPORTED, "KAI_SEQUENCER=device is not supported: the sequencer runs on the host");
   }
-  void *args[] = {(void *)&p};
+  if (e->cfg.shard_count > kShmRanks) return e->fail(KAI_ERR_UNSUPPORTED, "more GPUs than the exchange segment holds");
+  const int batching = getenv("KAI_NO_BATCHING") ? 0 : 1;
+  // one reduced answer line and one merged list per GPU; with several GPUs they live in the shared segment
+  unsigned long long *lines = e->cfg.shard_count > 1 ? e->shm_dev : e->h_slots;
+  unsigned long long *mm_lines = e->cfg.shard_count > 1 ? e->shm_dev + (size_t)2 * kMaxGrid * kSlotWords : e->h_mm;
+  p.h_slot = lines + (size_t)e->cfg.shard_rank * kSlotWords;
+  p.h_mmslot = mm_lines + (size_t)e->cfg.shard_rank * kSlotWords;
+  p.h_clist = e->cfg.shard_count > 1 ? e->shm_dev + shm_clist_offset_words() + (size_t)e->cfg.shard_rank * 2 * kCListWords : e->h_clist;
+  p.topm = (batching && !getenv("KAI_NO_TOPM")) ? 1 : 0;
+  p.scanners = e->lgrid;
+  p.nodes_per_cta = e->lnpc;
+  p.d_list = e->d_list;  // the scanners' top-M lines stay on the device; k_merge_cluster merges them
+  p.g_tiles = e->g_tiles;
+  p.g_tile_stride = e->ltile_stride;
+  p.tile_bytes = e->ltile_bytes;  // the scanners stage their tile in shared memory for a sweep
+  p.g_scan_state = e->g_scan_state;
+  p.ticket = e->ticket;
+  p.mm_result = e->mm_result;
+  p.spin_log2 = 22;
+  {
+    int per_sm = 0;
+    CK(cudaFuncSetAttribute(k_record, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)e->ltile_bytes));
+    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_record, kThreads, e->ltile_bytes));
+    p.fused_in_kernel = (per_sm * e->num_sms >= e->lgrid && !getenv("KAI_NO_FUSED_LAUNCH")) ? 1 : 0;
+  }
+  const unsigned int seq0 = e->seq;
   CK(cudaMemsetAsync(e->counters, 0, sizeof(long long) * 48, e->stream));
   cudaEventRecord(e->ev[2], e->stream);
   if (e->J > 0) k_prep_jobs<<<std::min(e->num_sms * 8, (e->J + 255) / 256), 256, 0, e->stream>>>(e->ds, 1, 1);
   if (e->Q > 0) k_prep_queues<<<e->Q, 256, 0, e->stream>>>(e->ds);
   long long c[48];
   memset(c, 0, sizeof(c));
-  if (host_mode) {
-    // host mirror of everything the open-session / prepare kernels produced
-    CK(cudaMemcpyAsync(e->stage.host + e->dev_only_begin, e->dsnap.base + e->dev_only_begin, e->dev_only_bytes,
-                       cudaMemcpyDeviceToHost, e->stream));
-    const bool feed_mirror = solver_action || e->topo.any() || e->cfg.shard_count > 1;
-    const bool refresh_mirror = feed_mirror && !e->mirror_valid;
-    if (refresh_mirror) e->topo.live = false;  // the incremental per-domain state is rebuilt from the re-read tables
-    if (refresh_mirror) {  // a device-sequenced action ran before: re-read the node tables (one GPU)
-      e->h_tmp.resize((size_t)2 * e->R * e->N);
-      if (e->N > 0) {
-        CK(cudaMemcpyAsync(e->h_tmp.data(), e->ds.idle, sizeof(double) * (size_t)e->R * e->N, cudaMemcpyDeviceToHost, e->stream));
-        CK(cudaMemcpyAsync(e->h_tmp.data() + (size_t)e->R * e->N, e->ds.rel, sizeof(double) * (size_t)e->R * e->N, cudaMemcpyDeviceToHost, e->stream));
-      }
+  // host mirror of everything the open-session / prepare kernels produced
+  CK(cudaMemcpyAsync(e->stage.host + e->dev_only_begin, e->dsnap.base + e->dev_only_begin, e->dev_only_bytes,
+                     cudaMemcpyDeviceToHost, e->stream));
+  const bool feed_mirror = solver_action || e->topo.any() || e->cfg.shard_count > 1;
+  const bool refresh_mirror = feed_mirror && !e->mirror_valid;
+  if (refresh_mirror) e->topo.live = false;  // the incremental per-domain state is rebuilt from the re-read tables
+  if (refresh_mirror) {  // an allocate that did not feed the mirror ran before: re-read the node tables (one GPU)
+    e->h_tmp.resize((size_t)2 * e->R * e->N);
+    if (e->N > 0) {
+      CK(cudaMemcpyAsync(e->h_tmp.data(), e->ds.idle, sizeof(double) * (size_t)e->R * e->N, cudaMemcpyDeviceToHost, e->stream));
+      CK(cudaMemcpyAsync(e->h_tmp.data() + (size_t)e->R * e->N, e->ds.rel, sizeof(double) * (size_t)e->R * e->N, cudaMemcpyDeviceToHost, e->stream));
     }
-    cudaEventRecord(e->ev_mirror, e->stream);
-    if (launch_mode) {
-      CK(cudaFuncSetAttribute(k_record, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)e->lsmem_bytes));
-      e->lp = p;
-      e->record_launches = 0;
-      LaunchRec load;
-      memset(&load, 0, sizeof(load));
-      load.dw[0] = (unsigned long long)DK_LOAD;
-      load.seq = p.seq0;
-      if (!engine_launch_record(e, load)) return e->cuda_fail(cudaGetLastError(), "k_record (tile load)");
-    } else {
-      CK(cudaLaunchCooperativeKernel((const void *)k_action, dim3(e->grid), dim3(kThreads), args, e->smem_bytes, e->stream));
-      cudaEventRecord(e->ev[3], e->stream);
-    }
-    // wait for the mirror copy only (the kernel keeps running): event-free trick = query the D2H through an event
-    cudaEvent_t mirror_done = e->ev[4];
-    (void)mirror_done;
-    // the D2H above precedes the kernel in stream order; its completion is observed by polling a sentinel
-    // written last: simplest robust way is a second stream-ordered event recorded before the launch.
-    // (see below: ev_mirror)
-    HostBackend &hb = e->hb;
-    hb.h_rec = e->h_rec;
-    hb.h_delta = e->h_delta;
-    hb.h_slots = e->cfg.shard_count > 1 ? e->shm_base : e->h_slots;
-    hb.h_mm = e->cfg.shard_count > 1 ? e->shm_base + (size_t)2 * kMaxGrid * kSlotWords : e->h_mm;
-    hb.n_scanners = e->cfg.shard_count;  // the relay CTA of every GPU reduces its scanners' answers: one line per GPU
-    hb.topm = p.topm;
-    hb.prof = getenv("KAI_PROFILE") != nullptr;
-    for (int i = 0; i < 8; i++) hb.t_sec[i] = 0;
-    hb.h_list = e->cfg.shard_count > 1 ? e->shm_base + (size_t)2 * 2 * kMaxGrid * kSlotWords : e->h_list;
-    hb.n_list_scanners = e->cfg.shard_count * (e->grid - 1);
-    hb.launch_mode = launch_mode;
-    hb.launch_fn = &engine_launch_record;
-    hb.launch_ctx = e;
-    hb.launches = 0;
-    hb.t_launch = 0;
-    hb.n_ranks = e->cfg.shard_count;
-    hb.h_clist = e->cfg.shard_count > 1 ? e->shm_base + shm_clist_offset_words() : e->h_clist;
-    hb.listed = 0;
-    hb.batch_is_single = false;
-    hb.list_yield_ema = 8.0;
-    hb.list_served = -1;
-    hb.single_streak = 0;
-    hb.single_sweeps = 0;
-    hb.n_flush = hb.n_topo_jobs = hb.n_topo_domains = 0;
-    hb.t_topo[0] = hb.t_topo[1] = hb.t_topo[2] = 0;
-    hb.list_invalidate();
-    hb.batching = p.batching;
-    hb.failed = false;
-    hb.gang_fast = getenv("KAI_NO_GANG_FAST") == nullptr;
-    hb.gang_bulk = hb.gang_replayed = hb.gang_failed = 0;
-    hb.rank_to_node = e->rank_to_node_h.data();
-    const double t_mirror0 = HostBackend::now();
-    CK(cudaEventSynchronize(e->ev_mirror));
-    if (refresh_mirror && !e->h_tmp.empty()) {  // re-read tables -> node-major mirror
-      for (int n = 0; n < e->N; n++)
-        for (int r = 0; r < e->R; r++) {
-          e->h_mirror[(size_t)n * 2 * e->R + r] = e->h_tmp[(size_t)r * e->N + n];
-          e->h_mirror[(size_t)n * 2 * e->R + e->R + r] = e->h_tmp[(size_t)(e->R + r) * e->N + n];
-        }
-    }
-    if (feed_mirror) e->mirror_valid = true;  // from here on the host-sequenced deltas keep it in step
-    const double t_mirror1 = HostBackend::now();
-    // ---- sequencer state on the host ----
-    const DevSnap &hs = e->hs;
-    const int Q = e->Q, J = e->J;
-    e->hot_host.assign(e->hot_bytes + 64, 0);
-    Seq &seq = hb.seq;
-    Ctl &ctl = hb.ctl;
-    memset(&ctl, 0, sizeof(ctl));
-    memset(&seq, 0, sizeof(seq));
-    {
-      unsigned char *h = e->hot_host.data();
-      auto take_from = [](unsigned char *&base, size_t bytes) {
-        unsigned char *r = base;
-        base += (bytes + 15) & ~(size_t)15;
-        return r;
-      };
-      Replica &rp = seq.rp;
-      rp.q_alloc = (double *)take_from(h, sizeof(double) * QR * Q);
-      rp.q_alloc_np = (double *)take_from(h, sizeof(double) * QR * Q);
-      rp.qkey = (QKey *)take_from(h, sizeof(QKey) * Q);
-      rp.leaf_head = (int *)take_from(h, sizeof(int) * Q);
-      rp.leaf_end = (int *)take_from(h, sizeof(int) * Q);
-      rp.ovl_len = (int *)take_from(h, sizeof(int) * Q);
-      rp.child_len = (int *)take_from(h, sizeof(int) * Q);
-      rp.child_heap = (int *)take_from(h, sizeof(int) * Q);
-      rp.root_heap = (int *)take_from(h, sizeof(int) * (hs.n_top + 1));
-      rp.qn_flags = (unsigned char *)take_from(h, Q);
-      rp.touched = (unsigned int *)take_from(h, sizeof(unsigned int) * ((J + 31) / 32 + 1));
-      rp.t_status = hs.t_status;
-      rp.t_node = hs.t_node;
-      rp.t_node_status = hs.t_node_status;
-      rp.t_virtual = hs.t_virtual;
-      rp.ps_active_alloc = hs.ps_cnt0;
-      rp.ps_pending = hs.ps_cnt0 + hs.S;
-      rp.ps_pipelined = hs.ps_cnt0 + 2 * hs.S;
-      rp.j_req = hs.j_req;
-      rp.j_req_valid = hs.j_req_valid;
-      rp.j_key = hs.j_key0;
-      rp.leaf_heap = hs.leaf_sorted;
-      rp.ops = hs.ops;
-      rp.tta = hs.tta;
-      rp.ps_order = hs.ps_order;
-      for (int i = 0; i < QR * Q; i++) {
-        rp.q_alloc[i] = hs.q_alloc[i];
-        rp.q_alloc_np[i] = hs.q_alloc_np[i];
-      }
-      for (int i = 0; i < Q; i++) {
-        int b = hs.q_job_begin[i];
-        rp.leaf_head[i] = b;
-        rp.leaf_end[i] = b + (hs.q_nchildren[i] == 0 ? hs.leaf_count[i] : 0);
-      }
-    }
-    seq.s = &e->hs;
-    seq.cfg = &e->cfg;
-    seq.p = &p;
-    seq.delta_base = e->h_delta;
-    seq.host_backend = &hb;
-    // The mirror is fed by the delta stream whenever something will read it: solver actions, topology, several GPUs.
-    // A plain single-GPU allocate skips that (one cache line per placement) and marks the mirror stale instead; a
-    // later solver action of the cycle re-reads the node tables from the device.
-    seq.mirror = feed_mirror ? e->h_mirror.data() : nullptr;
-    if (!feed_mirror) e->mirror_valid = false;
-    e->topo.mirror = e->h_mirror.data();
-    e->topo.t_req = hs.t_req;
-    e->topo.t_podset = hs.t_podset;
-    seq.topology = e->topo.any() ? &e->topo : nullptr;
-    seq.on_node_changed = &TopologyHost::node_changed_hook;
-    e->topo.reset_gpu_state();
-    seq.ctl = &ctl;
-    seq.ops_cap = e->ops_cap;
-    seq.batching = p.batching;
-    seq.is_cta0 = true;
-    e->r_visits.assign((size_t)e->visits_cap, kai_job_visit{0, 0});
-    seq.visits = e->r_visits.data();
-    seq.visits_cap = e->visits_cap;
-    ctl.trk[0].dirty = ctl.trk[1].dirty = 1;
-    ctl.trk[0].mn = ctl.trk[1].mn = DBL_MAX;
-    ctl.dec.nominated = ctl.dec.pred_class = -1;
-    ctl.dec.task = -1;
-    ctl.ctx_job = ctl.ctx_ps = -1;
-    ctl.seq = p.seq0;
-    long long solver_scenarios = 0, solver_topk = 0, solver_host_sweeps = 0, solver_host_topk = 0;
-    if (!solver_action) {
-      hb.run_allocate();
-    } else {
-      const int T = e->T;
-      if ((int)e->on_other_node.size() != T) {
-        e->on_other_node.assign(T, -1);
-        e->on_other_status.assign(T, 0);
-      }
-      double t_begin = HostBackend::now();
-      Solver solver(hb, e->solver_scratch, e->on_other_node, e->on_other_status, e->on_extra);
-      solver.use_signatures = e->cfg.use_scheduling_signatures != 0;
-      solver.job_signature = e->job_signature.empty() ? nullptr : e->job_signature.data();
-      solver.q_preempt_mrt = e->q_preempt_mrt.empty() ? nullptr : e->q_preempt_mrt.data();
-      solver.q_reclaim_mrt = e->q_reclaim_mrt.empty() ? nullptr : e->q_reclaim_mrt.data();
-      solver.j_last_start = e->j_last_start.empty() ? nullptr : e->j_last_start.data();
-      solver.j_stale_since = e->j_stale_since.empty() ? nullptr : e->j_stale_since.data();
-      solver.now_s = e->now_s;
-      const double t_ctor = HostBackend::now();
-      if (action == KAI_ACTION_RECLAIM)
-        solver.run_reclaim();
-      else if (action == KAI_ACTION_PREEMPT)
-        solver.run_preempt();
-      else if (action == KAI_ACTION_STALEGANGEVICTION)
-        solver.run_stale_gang_eviction();
-      else
-        solver.run_consolidation();
-      hb.publish(DK_DONE);
-      const double t_end = HostBackend::now();
-      hb.t_total = t_end - t_begin;
-      if (getenv("KAI_PROFILE"))
-        fprintf(stderr, "[kai] solver host profile: %lld simulations; sweeps %.1f ms, simulation set-up %.1f ms, evicting recorded victims %.1f ms, victims queues %.1f ms\n",
-                solver.simulations, solver.t_sweeps * 1e3, solver.t_sim_setup * 1e3, solver.t_evict * 1e3, solver.t_victims_queue * 1e3);
-      if (getenv("KAI_PROFILE"))
-        fprintf(stderr, "[kai] solver host profile: scenario loop: victims pop %.1f ms, tasks_to_evict %.1f, add potential %.1f, filter %.1f, filter init (top-k sweep) %.1f, by-pod solve %.1f\n",
-                solver.t_vq_pop * 1e3, solver.t_tte * 1e3, solver.t_addp * 1e3, solver.t_filter * 1e3, solver.t_finit * 1e3, solver.t_bypod * 1e3);
-      if (getenv("KAI_PROFILE"))
-        fprintf(stderr, "[kai] solver host profile: victims queues: %lld built (leaf tops %.2f ms), %lld copied (%.2f ms)\n",
-                solver.n_vq_build, solver.t_vq_top * 1e3, solver.n_vq_copy, solver.t_vq_copy * 1e3);
-      solver_scenarios = solver.scenarios;
-      solver_topk = solver.topk_sweeps;
-      solver_host_sweeps = solver.host_sweeps;
-      solver_host_topk = solver.host_topks;
-      // one status per task for the allocate path: the entry on the task's current node; the other entry persists.
-      // Only tasks the action changed (slot_list) and tasks with entries beyond two slots can need it: for any other
-      // task slot 0 is the snapshot's, on its current node with its current node status.
-      const double t_teardown = HostBackend::now();
-      SolverScratch &scr = e->solver_scratch;
-      std::vector<int> &n0 = scr.n0, &s0 = scr.s0;
-      for (auto &x : e->on_extra) {  // the entry on the task's current node belongs in slot 0
-        const int t = x[0], cur = hs.t_node[t];
-        solver.take_slot(t);
-        if (x[1] == cur && n0[t] != cur && e->on_other_node[t] != cur) {
-          if (n0[t] < 0) {
-            n0[t] = x[1];
-            s0[t] = x[2];
-            x[0] = -1;
-          } else {
-            std::swap(n0[t], x[1]);
-            std::swap(s0[t], x[2]);
-          }
-        }
-      }
-      e->on_extra.erase(std::remove_if(e->on_extra.begin(), e->on_extra.end(), [](const std::array<int, 3> &x) { return x[0] < 0; }),
-                        e->on_extra.end());
-      std::sort(scr.slot_list.begin(), scr.slot_list.end());  // ascending task order, as a scan of every task
-      for (int t : scr.slot_list) {
-        int cur = hs.t_node[t];
-        if (n0[t] >= 0 && n0[t] != cur && e->on_other_node[t] == cur) {
-          std::swap(n0[t], e->on_other_node[t]);
-          std::swap(s0[t], e->on_other_status[t]);
-        }
-        if (n0[t] >= 0 && n0[t] == cur)
-          hs.t_node_status[t] = s0[t];
-        else if (n0[t] >= 0) {  // only a stale entry on another node: it persists as "other" (or beyond the two slots)
-          if (e->on_other_node[t] < 0) {
-            e->on_other_node[t] = n0[t];
-            e->on_other_status[t] = s0[t];
-          } else {
-            e->on_extra.push_back({t, n0[t], s0[t]});
-          }
-        }
-      }
-      if (getenv("KAI_PROFILE"))
-        fprintf(stderr, "[kai] solver set-up / teardown: kai_engine_run entry to solver start %.2f ms (before the mirror wait %.2f, "
-                "mirror wait + refresh %.2f, sequencer state %.2f, Solver construction + scratch %.2f, prepare() %.2f); solver end "
-                "to the action's end event %.2f ms (task-slot reconciliation over %zu tasks %.2f)\n",
-                (t_ctor - t_entry) * 1e3 + solver.t_prepare * 1e3, (t_mirror0 - t_entry) * 1e3, (t_mirror1 - t_mirror0) * 1e3,
-                (t_begin - t_mirror1) * 1e3, (t_ctor - t_begin) * 1e3, solver.t_prepare * 1e3, (HostBackend::now() - t_end) * 1e3,
-                scr.slot_list.size(), (HostBackend::now() - t_teardown) * 1e3);
-    }
-    if (launch_mode) cudaEventRecord(e->ev[3], e->stream);  // after the DONE launch: the action's span on the device
-    CK(cudaStreamSynchronize(e->stream));
-    if (launch_mode) CK(cudaGetLastError());
-    if (solver_action && getenv("KAI_PROFILE"))
-      fprintf(stderr, "[kai] solver: %lld scenarios simulated, %lld node sweeps, %lld top-k sweeps, %lld minmax exchanges, "
-              "%lld restricted sweeps and %lld top-k lists answered on the host\n",
-              solver_scenarios, seq.sweeps, solver_topk, seq.minmax_exchanges, solver_host_sweeps, solver_host_topk);
-    {
-      long long cd[48];
-      CK(cudaMemcpy(cd, e->counters, sizeof(cd), cudaMemcpyDeviceToHost));
-      for (int i = 20; i < 32; i++) c[i] = cd[i];
-      for (int i = 32; i < 48; i++) c[i] = cd[i];
-    }
-    c[0] = seq.n_visits;
-    c[1] = seq.sweeps;
-    c[2] = seq.nodes_scanned;
-    c[3] = seq.pods_placed;
-    c[4] = seq.pods_evicted;
-    c[5] = seq.minmax_exchanges;
-    c[6] = seq.error;
-    c[7] = ctl.seq + 1;
-    c[15] = seq.batched + hb.listed;
-    if (hb.failed && c[24] == 0) c[24] = 99;
-    // session state back to the device copies (later actions' prepare kernels and the result download read them)
-    for (int i = 0; i < QR * Q; i++) {
-      hs.q_alloc[i] = seq.rp.q_alloc[i];
-      hs.q_alloc_np[i] = seq.rp.q_alloc_np[i];
-    }
-    auto up = [&](const void *hp, size_t bytes) {
-      size_t off = (const unsigned char *)hp - e->stage.host;
-      return cudaMemcpyAsync(e->dsnap.base + off, hp, bytes, cudaMemcpyHostToDevice, e->stream);
-    };
-    CK(up(hs.t_status, (size_t)e->T * 4));
-    CK(up(hs.t_node, (size_t)e->T * 4));
-    CK(up(hs.t_node_status, (size_t)e->T * 4));
-    CK(up(hs.t_virtual, (size_t)e->T));
-    CK(up(hs.q_alloc, (size_t)QR * Q * 8));
-    CK(up(hs.q_alloc_np, (size_t)QR * Q * 8));
-    if (e->visits_cap > 0 && seq.n_visits > 0)
-      CK(cudaMemcpyAsync(e->d_visits, e->r_visits.data(), sizeof(kai_job_visit) * (size_t)std::min<long long>(seq.n_visits, e->visits_cap),
-                         cudaMemcpyHostToDevice, e->stream));
-  } else {
-    CK(cudaLaunchCooperativeKernel((const void *)k_action, dim3(e->grid), dim3(kThreads), args, e->smem_bytes, e->stream));
-    cudaEventRecord(e->ev[3], e->stream);
-    CK(cudaMemcpyAsync(c, e->counters, sizeof(c), cudaMemcpyDeviceToHost, e->stream));
-    CK(cudaStreamSynchronize(e->stream));
   }
+  cudaEventRecord(e->ev_mirror, e->stream);
+  e->lp = p;
+  e->record_launches = 0;
+  LaunchRec load;
+  memset(&load, 0, sizeof(load));
+  load.dw[0] = (unsigned long long)DK_LOAD;
+  load.seq = seq0;
+  if (!engine_launch_record(e, load)) return e->cuda_fail(cudaGetLastError(), "k_record (tile load)");
+  HostBackend &hb = e->hb;
+  hb.h_slots = e->cfg.shard_count > 1 ? e->shm_base : e->h_slots;
+  hb.h_mm = e->cfg.shard_count > 1 ? e->shm_base + (size_t)2 * kMaxGrid * kSlotWords : e->h_mm;
+  hb.n_scanners = e->cfg.shard_count;  // the last CTA of every GPU reduces its scanners' answers: one line per GPU
+  hb.topm = p.topm;
+  hb.prof = getenv("KAI_PROFILE") != nullptr;
+  for (int i = 0; i < 8; i++) hb.t_sec[i] = 0;
+  hb.launch_fn = &engine_launch_record;
+  hb.launch_ctx = e;
+  hb.launches = 0;
+  hb.t_launch = 0;
+  hb.n_ranks = e->cfg.shard_count;
+  hb.h_clist = e->cfg.shard_count > 1 ? e->shm_base + shm_clist_offset_words() : e->h_clist;
+  hb.listed = 0;
+  hb.batch_is_single = false;
+  hb.list_yield_ema = 8.0;
+  hb.list_served = -1;
+  hb.single_streak = 0;
+  hb.single_sweeps = 0;
+  hb.n_flush = hb.n_topo_jobs = hb.n_topo_domains = 0;
+  hb.t_topo[0] = hb.t_topo[1] = hb.t_topo[2] = 0;
+  hb.list_invalidate();
+  hb.batching = batching;
+  hb.failed = false;
+  hb.gang_fast = getenv("KAI_NO_GANG_FAST") == nullptr;
+  hb.gang_bulk = hb.gang_replayed = hb.gang_failed = 0;
+  hb.rank_to_node = e->rank_to_node_h.data();
+  const double t_mirror0 = HostBackend::now();
+  CK(cudaEventSynchronize(e->ev_mirror));
+  if (refresh_mirror && !e->h_tmp.empty()) {  // re-read tables -> node-major mirror
+    for (int n = 0; n < e->N; n++)
+      for (int r = 0; r < e->R; r++) {
+        e->h_mirror[(size_t)n * 2 * e->R + r] = e->h_tmp[(size_t)r * e->N + n];
+        e->h_mirror[(size_t)n * 2 * e->R + e->R + r] = e->h_tmp[(size_t)(e->R + r) * e->N + n];
+      }
+  }
+  if (feed_mirror) e->mirror_valid = true;  // from here on the host-sequenced deltas keep it in step
+  const double t_mirror1 = HostBackend::now();
+  // ---- sequencer state on the host ----
+  const DevSnap &hs = e->hs;
+  const int Q = e->Q, J = e->J;
+  e->hot_host.assign(e->hot_bytes + 64, 0);
+  Seq &seq = hb.seq;
+  Ctl &ctl = hb.ctl;
+  memset(&ctl, 0, sizeof(ctl));
+  memset(&seq, 0, sizeof(seq));
+  {
+    unsigned char *h = e->hot_host.data();
+    auto take_from = [](unsigned char *&base, size_t bytes) {
+      unsigned char *r = base;
+      base += (bytes + 15) & ~(size_t)15;
+      return r;
+    };
+    Replica &rp = seq.rp;
+    rp.q_alloc = (double *)take_from(h, sizeof(double) * QR * Q);
+    rp.q_alloc_np = (double *)take_from(h, sizeof(double) * QR * Q);
+    rp.qkey = (QKey *)take_from(h, sizeof(QKey) * Q);
+    rp.leaf_head = (int *)take_from(h, sizeof(int) * Q);
+    rp.leaf_end = (int *)take_from(h, sizeof(int) * Q);
+    rp.ovl_len = (int *)take_from(h, sizeof(int) * Q);
+    rp.child_len = (int *)take_from(h, sizeof(int) * Q);
+    rp.child_heap = (int *)take_from(h, sizeof(int) * Q);
+    rp.root_heap = (int *)take_from(h, sizeof(int) * (hs.n_top + 1));
+    rp.qn_flags = (unsigned char *)take_from(h, Q);
+    rp.touched = (unsigned int *)take_from(h, sizeof(unsigned int) * ((J + 31) / 32 + 1));
+    rp.t_status = hs.t_status;
+    rp.t_node = hs.t_node;
+    rp.t_node_status = hs.t_node_status;
+    rp.t_virtual = hs.t_virtual;
+    rp.ps_active_alloc = hs.ps_cnt0;
+    rp.ps_pending = hs.ps_cnt0 + hs.S;
+    rp.ps_pipelined = hs.ps_cnt0 + 2 * hs.S;
+    rp.j_req = hs.j_req;
+    rp.j_req_valid = hs.j_req_valid;
+    rp.j_key = hs.j_key0;
+    rp.leaf_heap = hs.leaf_sorted;
+    rp.ops = hs.ops;
+    rp.tta = hs.tta;
+    rp.ps_order = hs.ps_order;
+    for (int i = 0; i < QR * Q; i++) {
+      rp.q_alloc[i] = hs.q_alloc[i];
+      rp.q_alloc_np[i] = hs.q_alloc_np[i];
+    }
+    for (int i = 0; i < Q; i++) {
+      int b = hs.q_job_begin[i];
+      rp.leaf_head[i] = b;
+      rp.leaf_end[i] = b + (hs.q_nchildren[i] == 0 ? hs.leaf_count[i] : 0);
+    }
+  }
+  seq.s = &e->hs;
+  seq.cfg = &e->cfg;
+  seq.delta_base = e->h_delta;
+  seq.host_backend = &hb;
+  // The mirror is fed by the delta stream whenever something will read it: solver actions, topology, several GPUs.
+  // A plain single-GPU allocate skips that (one cache line per placement) and marks the mirror stale instead; a
+  // later solver action of the cycle re-reads the node tables from the device.
+  seq.mirror = feed_mirror ? e->h_mirror.data() : nullptr;
+  if (!feed_mirror) e->mirror_valid = false;
+  e->topo.mirror = e->h_mirror.data();
+  e->topo.t_req = hs.t_req;
+  e->topo.t_podset = hs.t_podset;
+  seq.topology = e->topo.any() ? &e->topo : nullptr;
+  seq.on_node_changed = &TopologyHost::node_changed_hook;
+  e->topo.reset_gpu_state();
+  seq.ctl = &ctl;
+  seq.ops_cap = e->ops_cap;
+  seq.batching = batching;
+  e->r_visits.assign((size_t)e->visits_cap, kai_job_visit{0, 0});
+  seq.visits = e->r_visits.data();
+  seq.visits_cap = e->visits_cap;
+  ctl.trk[0].dirty = ctl.trk[1].dirty = 1;
+  ctl.trk[0].mn = ctl.trk[1].mn = DBL_MAX;
+  ctl.dec.nominated = ctl.dec.pred_class = -1;
+  ctl.dec.task = -1;
+  ctl.ctx_job = ctl.ctx_ps = -1;
+  ctl.seq = seq0;
+  long long solver_scenarios = 0, solver_topk = 0, solver_host_sweeps = 0, solver_host_topk = 0;
+  if (!solver_action) {
+    hb.run_allocate();
+  } else {
+    const int T = e->T;
+    if ((int)e->on_other_node.size() != T) {
+      e->on_other_node.assign(T, -1);
+      e->on_other_status.assign(T, 0);
+    }
+    double t_begin = HostBackend::now();
+    Solver solver(hb, e->solver_scratch, e->on_other_node, e->on_other_status, e->on_extra);
+    solver.use_signatures = e->cfg.use_scheduling_signatures != 0;
+    solver.job_signature = e->job_signature.empty() ? nullptr : e->job_signature.data();
+    solver.q_preempt_mrt = e->q_preempt_mrt.empty() ? nullptr : e->q_preempt_mrt.data();
+    solver.q_reclaim_mrt = e->q_reclaim_mrt.empty() ? nullptr : e->q_reclaim_mrt.data();
+    solver.j_last_start = e->j_last_start.empty() ? nullptr : e->j_last_start.data();
+    solver.j_stale_since = e->j_stale_since.empty() ? nullptr : e->j_stale_since.data();
+    solver.now_s = e->now_s;
+    const double t_ctor = HostBackend::now();
+    if (action == KAI_ACTION_RECLAIM)
+      solver.run_reclaim();
+    else if (action == KAI_ACTION_PREEMPT)
+      solver.run_preempt();
+    else if (action == KAI_ACTION_STALEGANGEVICTION)
+      solver.run_stale_gang_eviction();
+    else
+      solver.run_consolidation();
+    hb.publish(DK_DONE);
+    const double t_end = HostBackend::now();
+    hb.t_total = t_end - t_begin;
+    if (getenv("KAI_PROFILE"))
+      fprintf(stderr, "[kai] solver host profile: %lld simulations; sweeps %.1f ms, simulation set-up %.1f ms, evicting recorded victims %.1f ms, victims queues %.1f ms\n",
+              solver.simulations, solver.t_sweeps * 1e3, solver.t_sim_setup * 1e3, solver.t_evict * 1e3, solver.t_victims_queue * 1e3);
+    if (getenv("KAI_PROFILE"))
+      fprintf(stderr, "[kai] solver host profile: scenario loop: victims pop %.1f ms, tasks_to_evict %.1f, add potential %.1f, filter %.1f, filter init (top-k sweep) %.1f, by-pod solve %.1f\n",
+              solver.t_vq_pop * 1e3, solver.t_tte * 1e3, solver.t_addp * 1e3, solver.t_filter * 1e3, solver.t_finit * 1e3, solver.t_bypod * 1e3);
+    if (getenv("KAI_PROFILE"))
+      fprintf(stderr, "[kai] solver host profile: victims queues: %lld built (leaf tops %.2f ms), %lld copied (%.2f ms)\n",
+              solver.n_vq_build, solver.t_vq_top * 1e3, solver.n_vq_copy, solver.t_vq_copy * 1e3);
+    solver_scenarios = solver.scenarios;
+    solver_topk = solver.topk_sweeps;
+    solver_host_sweeps = solver.host_sweeps;
+    solver_host_topk = solver.host_topks;
+    // one status per task for the allocate path: the entry on the task's current node; the other entry persists.
+    // Only tasks the action changed (slot_list) and tasks with entries beyond two slots can need it: for any other
+    // task slot 0 is the snapshot's, on its current node with its current node status.
+    const double t_teardown = HostBackend::now();
+    SolverScratch &scr = e->solver_scratch;
+    std::vector<int> &n0 = scr.n0, &s0 = scr.s0;
+    for (auto &x : e->on_extra) {  // the entry on the task's current node belongs in slot 0
+      const int t = x[0], cur = hs.t_node[t];
+      solver.take_slot(t);
+      if (x[1] == cur && n0[t] != cur && e->on_other_node[t] != cur) {
+        if (n0[t] < 0) {
+          n0[t] = x[1];
+          s0[t] = x[2];
+          x[0] = -1;
+        } else {
+          std::swap(n0[t], x[1]);
+          std::swap(s0[t], x[2]);
+        }
+      }
+    }
+    e->on_extra.erase(std::remove_if(e->on_extra.begin(), e->on_extra.end(), [](const std::array<int, 3> &x) { return x[0] < 0; }),
+                      e->on_extra.end());
+    std::sort(scr.slot_list.begin(), scr.slot_list.end());  // ascending task order, as a scan of every task
+    for (int t : scr.slot_list) {
+      int cur = hs.t_node[t];
+      if (n0[t] >= 0 && n0[t] != cur && e->on_other_node[t] == cur) {
+        std::swap(n0[t], e->on_other_node[t]);
+        std::swap(s0[t], e->on_other_status[t]);
+      }
+      if (n0[t] >= 0 && n0[t] == cur)
+        hs.t_node_status[t] = s0[t];
+      else if (n0[t] >= 0) {  // only a stale entry on another node: it persists as "other" (or beyond the two slots)
+        if (e->on_other_node[t] < 0) {
+          e->on_other_node[t] = n0[t];
+          e->on_other_status[t] = s0[t];
+        } else {
+          e->on_extra.push_back({t, n0[t], s0[t]});
+        }
+      }
+    }
+    if (getenv("KAI_PROFILE"))
+      fprintf(stderr, "[kai] solver set-up / teardown: kai_engine_run entry to solver start %.2f ms (before the mirror wait %.2f, "
+              "mirror wait + refresh %.2f, sequencer state %.2f, Solver construction + scratch %.2f, prepare() %.2f); solver end "
+              "to the action's end event %.2f ms (task-slot reconciliation over %zu tasks %.2f)\n",
+              (t_ctor - t_entry) * 1e3 + solver.t_prepare * 1e3, (t_mirror0 - t_entry) * 1e3, (t_mirror1 - t_mirror0) * 1e3,
+              (t_begin - t_mirror1) * 1e3, (t_ctor - t_begin) * 1e3, solver.t_prepare * 1e3, (HostBackend::now() - t_end) * 1e3,
+              scr.slot_list.size(), (HostBackend::now() - t_teardown) * 1e3);
+  }
+  cudaEventRecord(e->ev[3], e->stream);  // after the DONE launch: the action's span on the device
+  CK(cudaStreamSynchronize(e->stream));
+  CK(cudaGetLastError());
+  if (solver_action && getenv("KAI_PROFILE"))
+    fprintf(stderr, "[kai] solver: %lld scenarios simulated, %lld node sweeps, %lld top-k sweeps, %lld minmax exchanges, "
+            "%lld restricted sweeps and %lld top-k lists answered on the host\n",
+            solver_scenarios, seq.sweeps, solver_topk, seq.minmax_exchanges, solver_host_sweeps, solver_host_topk);
+  {
+    long long cd[48];
+    CK(cudaMemcpy(cd, e->counters, sizeof(cd), cudaMemcpyDeviceToHost));
+    for (int i = 24; i < 48; i++) c[i] = cd[i];
+  }
+  c[0] = seq.n_visits;
+  c[1] = seq.sweeps;
+  c[2] = seq.nodes_scanned;
+  c[3] = seq.pods_placed;
+  c[4] = seq.pods_evicted;
+  c[5] = seq.minmax_exchanges;
+  c[6] = seq.error;
+  c[7] = ctl.seq + 1;
+  c[15] = seq.batched + hb.listed;
+  if (hb.failed && c[24] == 0) c[24] = 99;
+  // session state back to the device copies (later actions' prepare kernels and the result download read them)
+  for (int i = 0; i < QR * Q; i++) {
+    hs.q_alloc[i] = seq.rp.q_alloc[i];
+    hs.q_alloc_np[i] = seq.rp.q_alloc_np[i];
+  }
+  auto up = [&](const void *hp, size_t bytes) {
+    size_t off = (const unsigned char *)hp - e->stage.host;
+    return cudaMemcpyAsync(e->dsnap.base + off, hp, bytes, cudaMemcpyHostToDevice, e->stream);
+  };
+  CK(up(hs.t_status, (size_t)e->T * 4));
+  CK(up(hs.t_node, (size_t)e->T * 4));
+  CK(up(hs.t_node_status, (size_t)e->T * 4));
+  CK(up(hs.t_virtual, (size_t)e->T));
+  CK(up(hs.q_alloc, (size_t)QR * Q * 8));
+  CK(up(hs.q_alloc_np, (size_t)QR * Q * 8));
+  if (e->visits_cap > 0 && seq.n_visits > 0)
+    CK(cudaMemcpyAsync(e->d_visits, e->r_visits.data(), sizeof(kai_job_visit) * (size_t)std::min<long long>(seq.n_visits, e->visits_cap),
+                       cudaMemcpyHostToDevice, e->stream));
   float ms = 0;
   cudaEventElapsedTime(&ms, e->ev[2], e->ev[3]);
   e->stats.action_ms = ms;
   e->stats.decisions = c[1];
   e->stats.nodes_scanned = c[2];
   e->stats.algorithmic_bytes = c[2] * ((2 * e->R + 1) * 8 + 4);
-  e->stats.kernel_launches += (launch_mode ? e->record_launches : 1) + (e->J > 0) + (e->Q > 0);
+  e->stats.kernel_launches += e->record_launches + (e->J > 0) + (e->Q > 0);
   e->seq = (unsigned int)c[7];
   if (getenv("KAI_PROFILE")) {
-    const char *nm[] = {"init", "pop", "prepare", "keycalc", "exchange", "apply", "finish"};
-    fprintf(stderr, "[kai] %s-sequenced action %.3f ms, %lld sweeps, %lld batched placements, %lld minmax exchanges, hot_in_smem=%d; CTA0 thread0 cycles:", host_mode ? "host" : "device", ms, c[1], c[15], c[5], (int)e->hot_in_smem);
-    for (int i = 0; i < 7; i++) fprintf(stderr, " %s=%lld", nm[i], c[8 + i]);
-    fprintf(stderr, " n_key=%lld tta=%lld popheap=%lld\n", c[16], c[17], c[18]);
-    if (host_mode)
-      fprintf(stderr, "[kai] host sequencer (%s transport, %lld record launches): total %.3f ms, of which waiting for sweeps %.3f ms (%.2f us per sweep)\n",
-              launch_mode ? "launch" : "persistent", launch_mode ? e->record_launches : 0LL, e->hb.t_total * 1e3, e->hb.t_exchange * 1e3,
-              c[1] ? e->hb.t_exchange * 1e6 / c[1] : 0.0);
-    if (host_mode && launch_mode) fprintf(stderr, "[kai] launch calls: %.3f ms on the host thread (%.2f us per record)\n", e->hb.t_launch * 1e3, e->hb.launches ? e->hb.t_launch * 1e6 / e->hb.launches : 0.0);
-    if (host_mode) fprintf(stderr, "[kai] sweeps answered with a single row (XB_SINGLE): %lld; FLUSH records %lld\n", e->hb.single_sweeps, e->hb.n_flush);
-    if (host_mode) fprintf(stderr, "[kai] fresh gangs: %lld committed in bulk, %lld replayed per task, %lld discarded\n", e->hb.gang_bulk, e->hb.gang_replayed, e->hb.gang_failed);
-    if (host_mode && e->hb.n_topo_jobs)
+    fprintf(stderr, "[kai] host-sequenced action %.3f ms, %lld sweeps, %lld batched placements, %lld minmax exchanges\n", ms, c[1], c[15], c[5]);
+    fprintf(stderr, "[kai] host sequencer (%lld record launches): total %.3f ms, of which waiting for sweeps %.3f ms (%.2f us per sweep)\n",
+            e->record_launches, e->hb.t_total * 1e3, e->hb.t_exchange * 1e3, c[1] ? e->hb.t_exchange * 1e6 / c[1] : 0.0);
+    fprintf(stderr, "[kai] launch calls: %.3f ms on the host thread (%.2f us per record)\n", e->hb.t_launch * 1e3, e->hb.launches ? e->hb.t_launch * 1e6 / e->hb.launches : 0.0);
+    fprintf(stderr, "[kai] sweeps answered with a single row (XB_SINGLE): %lld; FLUSH records %lld\n", e->hb.single_sweeps, e->hb.n_flush);
+    fprintf(stderr, "[kai] fresh gangs: %lld committed in bulk, %lld replayed per task, %lld discarded\n", e->hb.gang_bulk, e->hb.gang_replayed, e->hb.gang_failed);
+    if (e->hb.n_topo_jobs)
       fprintf(stderr, "[kai] topology: %lld constrained jobs with candidates, %lld domains tried; subSetNodesFn %.1f ms, score table %.1f ms, placing %.1f ms\n",
               e->hb.n_topo_jobs, e->hb.n_topo_domains, e->hb.t_topo[0] * 1e3, e->hb.t_topo[1] * 1e3, e->hb.t_topo[2] * 1e3);
-    if (host_mode)
-      fprintf(stderr, "[kai] host sequencer rdtsc Mcycles: pop %.2f admit %.2f place(+sweeps) %.2f finish %.2f loop %.2f\n",
+    fprintf(stderr, "[kai] host sequencer rdtsc Mcycles: pop %.2f admit %.2f place(+sweeps) %.2f finish %.2f loop %.2f\n",
               e->hb.t_sec[0] / 1e6, e->hb.t_sec[1] / 1e6, e->hb.t_sec[2] / 1e6, e->hb.t_sec[3] / 1e6, e->hb.t_sec[4] / 1e6);
-    if (host_mode && c[45] > 0)
-      fprintf(stderr, "[kai] %s: %lld cycles per list (%lld lists): load %lld, sort %lld, prefix + payload %lld, stream out %lld, fence + header %lld\n",
-              e->merge_cluster ? "k_merge_cluster" : "k_merge", c[44] / c[45], c[45], c[39] / c[45], c[46] / c[45], c[31] / c[45], c[47] / c[45], c[43] / c[45]);
-    if (host_mode && c[22] > 0)
-      fprintf(stderr, "[kai] relay CTA per record: forward %lld cycles, scanners+reduce %lld cycles (%lld records)\n",
-              c[20] / c[22], c[21] / c[22], c[22]);
-    if (host_mode && c[38] > 0)
-      fprintf(stderr, "[kai] scanner 0 per record (cycles): wait-for-record %lld (of which word-0 poll %lld), decode %lld, deltas %lld, scan %lld, scan+publish %lld\n",
-              c[33] / c[38], c[32] / c[38], c[34] / c[38], c[35] / c[38], c[36] / c[38], c[37] / c[38]);
-    if (host_mode && c[38] > 0)
+    if (c[45] > 0)
+      fprintf(stderr, "[kai] k_merge_cluster: %lld cycles per list (%lld lists): load %lld, sort %lld, prefix + payload + stream out + header %lld\n",
+              c[44] / c[45], c[45], c[39] / c[45], c[46] / c[45], c[31] / c[45]);
+    if (c[38] > 0)
+      fprintf(stderr, "[kai] scanner 0 per record (cycles): record words %lld, decode %lld, deltas %lld, scan %lld, scan+publish %lld\n",
+              c[33] / c[38], c[34] / c[38], c[35] / c[38], c[36] / c[38], c[37] / c[38]);
+    if (c[38] > 0)
       fprintf(stderr, "[kai] publish_candidate of scanner 0 (cycles per record): row+advance %lld, key %lld, events+pack %lld\n",
               c[40] / c[38], c[41] / c[38], c[42] / c[38]);
   }
   if (c[24] != 0) {
     char msg[256];
     snprintf(msg, sizeof(msg), "device protocol watchdog: wait code %lld seq %lld who %lld cta %lld (seq0 %u, end seq %lld)",
-             c[24], c[25], c[26], c[27], p.seq0, c[7]);
+             c[24], c[25], c[26], c[27], seq0, c[7]);
     e->loaded = false;
     std::string m2 = msg;
-    if (host_mode) {
-      char b2[96];
-      snprintf(b2, sizeof(b2), "; relay last forwarded kind %lld seq %lld; host trace:", c[23] >> 32, c[23] & 0xffffffff);
+    char b2[96];
+    m2 += "; host trace:";
+    unsigned int n0 = e->hb.trace_n > 16 ? e->hb.trace_n - 16 : 0;
+    for (unsigned int i = n0; i < e->hb.trace_n; i++) {
+      snprintf(b2, sizeof(b2), " (%u k%d nd%d)", e->hb.trace_seq[i & 63], e->hb.trace_kind[i & 63], e->hb.trace_nd[i & 63]);
       m2 += b2;
-      unsigned int n0 = e->hb.trace_n > 16 ? e->hb.trace_n - 16 : 0;
-      for (unsigned int i = n0; i < e->hb.trace_n; i++) {
-        snprintf(b2, sizeof(b2), " (%u k%d nd%d)", e->hb.trace_seq[i & 63], e->hb.trace_kind[i & 63], e->hb.trace_nd[i & 63]);
-        m2 += b2;
-      }
     }
     return e->fail(KAI_ERR_CUDA, m2);
   }
   if (c[6] == 2) return e->fail(KAI_ERR_UNSUPPORTED, "topology: more preferred-level domains than the score table holds (kDomBuckets)");
   if (c[6] == Solver::kSeqErrHostSweep) return e->fail(KAI_ERR_INVALID, e->hb.error_msg);
-  if (c[6] != 0) return e->fail(KAI_ERR_CUDA, "device sequencer overflow (statement log)");
+  if (c[6] != 0) return e->fail(KAI_ERR_CUDA, "sequencer overflow (statement log)");
   return download(e, out, c[0], c[3], c[4]);
 }
 
@@ -1580,19 +1452,16 @@ int kai_engine_time_sweeps(kai_engine *e, int n_launches, double *elapsed_ms, do
   memset(&p, 0, sizeof(p));
   p.s = e->ds;
   p.cfg = e->cfg;
-  p.action = KAI_ACTION_ALLOCATE;
-  p.grid = e->lgrid + 1;
+  p.scanners = e->lgrid;
   p.nodes_per_cta = e->lnpc;
   p.xbuf = e->xbuf;
   p.mmbuf = e->mmbuf;
   p.counters = e->counters;
   p.node_domain = e->d_node_domain;
   p.n_dom_levels = e->n_dom_levels;
-  p.mode = 2;
   p.spin_log2 = 22;
   p.topm = 1;
-  p.batching = 1;
-  p.h_list = e->d_list;
+  p.d_list = e->d_list;
   p.g_tiles = e->g_tiles;
   p.g_tile_stride = e->ltile_stride;
   p.g_scan_state = e->g_scan_state;
@@ -1601,10 +1470,8 @@ int kai_engine_time_sweeps(kai_engine *e, int n_launches, double *elapsed_ms, do
   p.h_slot = e->h_slots;
   p.h_mmslot = e->h_mm;
   p.h_clist = e->h_clist;
-  CK(cudaFuncSetAttribute(k_record, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)e->lsmem_bytes));
-  CK(cudaFuncSetAttribute(k_merge, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMergeSmemBytes));
+  CK(cudaFuncSetAttribute(k_record, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)e->ltile_bytes));
   p.tile_bytes = e->ltile_bytes;
-  p.hot_in_smem = e->ltile_bytes <= e->lsmem_bytes ? 1 : 0;
   e->lp = p;
   LaunchRec rec;
   memset(&rec, 0, sizeof(rec));
@@ -1634,19 +1501,11 @@ int kai_engine_time_sweeps(kai_engine *e, int n_launches, double *elapsed_ms, do
   cudaEventRecord(e->ev[0], e->stream);
   for (int i = 0; i < n_launches; i++) {
     rec.seq = e->seq + 1 + (unsigned int)i;
-    k_record<<<e->lgrid, kThreads, e->lsmem_bytes, e->stream>>>(e->lp, rec);
+    k_record<<<e->lgrid, kThreads, e->ltile_bytes, e->stream>>>(e->lp, rec);
   }
   cudaEventRecord(e->ev[1], e->stream);
-  {
-    const char *mk = getenv("KAI_MERGE");
-    e->merge_cluster = !(mk && strcmp(mk, "single") == 0);
-  }
-  for (int i = 0; i < n_launches; i++) {
-    if (e->merge_cluster)
-      k_merge_cluster<<<kMergeCtas, kMergeCtaThreads, kMergeCtaSmemBytes, e->stream>>>(e->lp, rec.seq, 1);
-    else
-      k_merge<<<1, kMergeThreads, kMergeSmemBytes, e->stream>>>(e->lp, rec.seq, 1);
-  }
+  for (int i = 0; i < n_launches; i++)
+    k_merge_cluster<<<kMergeCtas, kMergeCtaThreads, kMergeCtaSmemBytes, e->stream>>>(e->lp, rec.seq, 1);
   cudaEventRecord(e->ev[2], e->stream);
   CK(cudaStreamSynchronize(e->stream));
   CK(cudaGetLastError());

@@ -1,18 +1,13 @@
-// kai_host_seq.cuh — host backend of the sequencer (host-sequenced mode).
+// kai_host_seq.cuh — the host sequencer's allocate action and its exchange with the GPU.
 //
-// The sequencer source (kai_seq.cuh) is compiled for the host as well.  A CPU thread of libkaigpu.so runs it against a
-// host mirror of the session state and sends the GPU one decision record per node-table sweep:
-//   * launch transport (default): publish() = one k_record launch carrying the record in its kernel parameters; list
-//     answers come back as ONE merged, cut and sorted list per GPU (k_merge_cluster), single-row / min-max answers as one
-//     line reduced by the last CTA; the host waits on a sequence tag in pinned host memory;
-//   * persistent transport: the GPU runs k_action as a "scan server": CTA 0 relays the records the host writes into pinned
-//     mapped memory to the scanners' device-side record buffer, the scanners keep their node tiles in shared memory and
-//     answer every record with tagged 128-bit words written straight into pinned host memory.
+// A CPU thread of libkaigpu.so runs the sequencer (kai_seq.cuh) against a host mirror of the session state and sends
+// the GPU one decision record per node-table sweep: publish() = one k_record launch carrying the record in its kernel
+// parameters.  List answers come back as ONE merged, cut and sorted list per GPU (k_merge_cluster), single-row /
+// min-max answers as one line reduced by the last CTA; the host waits on a sequence tag in pinned host memory.
 //
-// Why: the pointer-chasing part of the cycle (heap pops, DRF keys, statement log) is a chain of dependent
-// L1/L2/shared-memory accesses per job (latencies in profiles/microbench) on a single GPU lane; a host core
-// serves the same chain from its caches far faster.  The O(N) work per allocateTask — the node sweep — stays
-// on the GPU in both modes.
+// Why: the pointer-chasing part of the cycle (heap pops, DRF keys, statement log) is a chain of dependent accesses per
+// job; a host core serves it from its caches far faster than one GPU lane (latencies in profiles/microbench).  The
+// O(N) work per allocateTask — the node sweep — stays on the GPU.
 #pragma once
 #include <algorithm>
 #include <chrono>
@@ -26,9 +21,7 @@
 namespace kai {
 
 struct HostBackend {
-  // pinned, device-mapped buffers
-  unsigned long long *h_rec = nullptr;    // [2][kDecWords][2]
-  unsigned long long *h_delta = nullptr;  // [2][kMaxDelta][2]
+  // pinned, device-mapped answer lines: one per GPU
   unsigned long long *h_slots = nullptr;  // [2][kMaxGrid][kSlotWords]
   unsigned long long *h_mm = nullptr;     // [2][kMaxGrid][kSlotWords]
   int n_scanners = 0;
@@ -42,16 +35,12 @@ struct HostBackend {
   long long spins = 0;
   double t_exchange = 0, t_total = 0;  // seconds: waiting for the GPU / whole action
   // ---- top-M candidate lists ----
-  unsigned long long *h_list = nullptr;  // [2][kListScanners][kListLines][kListLineWords]
   int topm = 0;
-  int n_list_scanners = 0;  // scanners of all GPUs
   struct ListCand {
     double score;
     uint32_t rank, flags;
     int node, cap, used;
     double Ig, Lg, Ic, Lc;
-    const unsigned long long *payload;
-    bool loaded;
   };
   std::vector<ListCand> list;
   size_t list_pos = 0, list_valid = 0;
@@ -89,8 +78,7 @@ struct HostBackend {
   unsigned int trace_seq[64];
   int trace_nd[64];
   unsigned int trace_n = 0;
-  // ---- launch transport: a record is a kernel launch (k_record), the answer one merged line / list per GPU ----
-  bool launch_mode = false;
+  // ---- a record is a kernel launch (k_record), the answer one merged line / list per GPU ----
   void *launch_ctx = nullptr;
   bool (*launch_fn)(void *ctx, const LaunchRec &rec) = nullptr;  // kai_engine.cu: enqueues the launch(es) of one record
   unsigned long long *h_clist = nullptr;  // [ranks][2][kCListWords] merged candidate lists (pinned / shared host memory)
@@ -105,27 +93,22 @@ struct HostBackend {
     trace_n++;
     close_delta(ctl, seq.delta_base);
     build_decision_words(ctl, kind, batching);
-    if (launch_mode) {
-      for (int i = 0; i < kDecWords; i++) lrec.dw[i] = ctl.dw[i];
-      lrec.seq = ctl.seq;
-      lrec.n_delta = ctl.n_delta;
-      const unsigned long long *dl = seq.delta_base + (size_t)(ctl.seq & 1) * kMaxDelta * 2;
-      for (int e = 0; e < ctl.n_delta; e++) {
-        lrec.dkey[e] = (unsigned int)(dl[2 * e] & 0xffffffffu);
-        lrec.dtask[e] = (unsigned int)(dl[2 * e] >> 32);
-        lrec.dcount[e] = (unsigned char)((dl[2 * e + 1] >> 32) & 0xffu);
-      }
-      launches++;
-      const double tl = prof ? now() : 0.0;
-      if (!launch_fn(launch_ctx, lrec)) failed = true;
-      if (prof) t_launch += now() - tl;
-      return;
+    for (int i = 0; i < kDecWords; i++) lrec.dw[i] = ctl.dw[i];
+    lrec.seq = ctl.seq;
+    lrec.n_delta = ctl.n_delta;
+    const unsigned long long *dl = seq.delta_base + (size_t)(ctl.seq & 1) * kMaxDelta * 2;
+    for (int e = 0; e < ctl.n_delta; e++) {
+      lrec.dkey[e] = (unsigned int)(dl[2 * e] & 0xffffffffu);
+      lrec.dtask[e] = (unsigned int)(dl[2 * e] >> 32);
+      lrec.dcount[e] = (unsigned char)((dl[2 * e + 1] >> 32) & 0xffu);
     }
-    unsigned long long *rec = h_rec + (size_t)(ctl.seq & 1) * kDecWords * 2;
-    for (int i = kDecWords - 1; i >= 0; i--) store_tagged(rec + 2 * i, ctl.dw[i], (unsigned long long)ctl.seq);
+    launches++;
+    const double tl = prof ? now() : 0.0;
+    if (!launch_fn(launch_ctx, lrec)) failed = true;
+    if (prof) t_launch += now() - tl;
   }
 
-  // gather the candidate slots (written by the scanners over PCIe as single 16-byte stores)
+  // gather the answer line of every GPU (written by its last CTA over PCIe as single 16-byte stores)
   void gather_candidates() {
     const unsigned int seq_no = ctl.seq;
     const unsigned long long *buf = h_slots + (size_t)(seq_no & 1) * kMaxGrid * kSlotWords;
@@ -184,11 +167,10 @@ struct HostBackend {
     ctl.n_delta = 0;
   }
 
-  // Gather the top-M answers of every scanner, merge them into one list in key order and mark the prefix that
-  // is provably the global order: entries strictly better than the last reported key of any scanner that has more
-  // fitting rows than it reported.
-  // launch transport: every GPU's last CTA has merged, cut and written its list; merge the lists of the ranks
-  void gather_list_merged() {
+  // Every GPU's k_merge_cluster has merged, cut and written its list: merge the lists of the ranks into one list in key
+  // order and mark the prefix that is provably the global order: entries strictly better than the last listed key of
+  // any GPU that has more fitting rows than it listed.
+  void gather_list() {
     const unsigned int seq_no = ctl.seq;
     list.clear();
     bool have_cut = false;
@@ -211,8 +193,6 @@ struct HostBackend {
         lc.node = rank_to_node[lc.rank];
         lc.cap = 1 + (int)((meta >> 24) & 0xffu);
         lc.used = 0;
-        lc.payload = nullptr;
-        lc.loaded = true;
         memcpy(&lc.Ig, &e[2], 8);
         memcpy(&lc.Lg, &e[3], 8);
         memcpy(&lc.Ic, &e[4], 8);
@@ -241,74 +221,10 @@ struct HostBackend {
         }
     list_pos = 0;
     list_more = have_cut;
-    list_tag = seq_no & 0xffffffu;
     ctl.seq = seq_no + 1;
     ctl.n_delta = 0;
     ctl.batch.valid = 0;
   }
-  void gather_list() {
-    if (launch_mode) return gather_list_merged();
-    const unsigned int seq_no = ctl.seq;
-    const unsigned int tag = seq_no & 0xffffffu;
-    const unsigned long long *base = h_list + (size_t)(seq_no & 1) * kListScanners * kListLines * kListLineWords;
-    list.clear();
-    bool have_cut = false;
-    double cut_score = 0;
-    uint32_t cut_rank = 0;
-    for (int c = 0; c < n_list_scanners && !failed; c++) {
-      const unsigned long long *lines = base + (size_t)c * kListLines * kListLineWords;
-      bool more = false;
-      double last_score = 0;
-      uint32_t last_rank = kRankNone;
-      for (int m = 0; m < kTopM; m++) {
-        unsigned long long hi;
-        if (!wait_word(lines + 2 * m + 1, [&](unsigned long long v) { return (unsigned int)(v >> 40) == tag; }, hi)) break;
-        unsigned long long lo = __atomic_load_n(lines + 2 * m, __ATOMIC_RELAXED);
-        uint32_t rk = (uint32_t)(hi & 0xffffffu);
-        uint32_t fl = (uint32_t)((hi >> 32) & 0xffu);
-        if (fl & LF_MORE) more = true;
-        if (rk == kRankNone) continue;
-        ListCand lc;
-        memcpy(&lc.score, &lo, 8);
-        lc.rank = rk;
-        lc.flags = fl;
-        lc.node = rank_to_node[rk];
-        lc.cap = 1 + (int)((hi >> 24) & 0xffu);
-        lc.used = 0;
-        lc.payload = lines + (size_t)(1 + m) * kListLineWords;
-        lc.loaded = false;
-        lc.Ig = lc.Lg = lc.Ic = lc.Lc = 0;
-        list.push_back(lc);
-        last_score = lc.score;
-        last_rank = rk;
-      }
-      if (more && last_rank != kRankNone) {  // an unseen row of this scanner can be at most this good
-        if (!have_cut || last_score > cut_score || (last_score == cut_score && last_rank < cut_rank)) {
-          have_cut = true;
-          cut_score = last_score;
-          cut_rank = last_rank;
-        }
-      }
-    }
-    std::sort(list.begin(), list.end(), [](const ListCand &a, const ListCand &b) {
-      return a.score > b.score || (a.score == b.score && a.rank < b.rank);
-    });
-    list_valid = list.size();
-    if (have_cut)
-      for (size_t i = 0; i < list.size(); i++)
-        if (!(list[i].score > cut_score || (list[i].score == cut_score && list[i].rank <= cut_rank))) {
-          list_valid = i;
-          break;
-        }
-    // the cut row itself was reported (it IS the last reported row of that scanner): it may be used, rows after it not
-    list_pos = 0;
-    list_more = have_cut;
-    list_tag = tag;
-    ctl.seq = seq_no + 1;
-    ctl.n_delta = 0;
-    ctl.batch.valid = 0;
-  }
-  unsigned int list_tag = 0;
   bool list_more = false;
   bool batch_is_single = false;  // ctl.batch comes from a single-winner answer (same-node repeats), not from a list
   double list_yield_ema = 8.0;   // pods served per list, recent average
@@ -417,7 +333,7 @@ struct HostBackend {
     gang_replayed++;
     return true;
   }
-  // seq_apply_winner / seq_apply_batched (kai_seq.cuh) with the placement routed through place()
+  // placement of a single-row answer / of the next same-node repeat, routed through place()
   void apply_winner_host(int t) {
     seq.sweeps++;
     seq.nodes_scanned += seq.s->N;
@@ -447,17 +363,6 @@ struct HostBackend {
     if (!list_available()) return false;
     ListCand &lc = list[list_pos];
     const Decision &d = ctl.dec;
-    if (!lc.loaded) {
-      const unsigned int tag = list_tag;  // the sweep that produced the list (a FLUSH may have advanced ctl.seq since)
-      double *dst[4] = {&lc.Ig, &lc.Lg, &lc.Ic, &lc.Lc};
-      for (int w = 0; w < 4; w++) {
-        unsigned long long hi;
-        if (!wait_word(lc.payload + 2 * w + 1, [&](unsigned long long v) { return (unsigned int)v == tag; }, hi)) return false;
-        unsigned long long lo = __atomic_load_n(lc.payload + 2 * w, __ATOMIC_RELAXED);
-        memcpy(dst[w], &lo, 8);
-      }
-      lc.loaded = true;
-    }
     const bool to_idle = (lc.flags & LF_TO_IDLE) != 0;
     bool scored_moved = false;
     for (int k = 0; k < 2; k++) {
@@ -690,24 +595,12 @@ struct HostBackend {
 
   void flush_deltas() {
     n_flush++;
-    publish(DK_FLUSH);
-    if (launch_mode) {  // stream order: the next launch sees these deltas applied; nothing to wait for
-      ctl.seq++;
-      ctl.n_delta = 0;
-      return;
-    }
-    const unsigned int seq_no = ctl.seq;
-    const unsigned long long *buf = h_slots + (size_t)(seq_no & 1) * kMaxGrid * kSlotWords;
-    const unsigned int tag = seq_no & 0xffffffu;
-    for (int c = 0; c < n_scanners; c++) {
-      unsigned long long hi;
-      if (!wait_word(buf + (size_t)c * kSlotWords + 1, [&](unsigned long long v) { return (unsigned int)(v >> 40) == tag; }, hi)) break;
-    }
-    ctl.seq = seq_no + 1;
+    publish(DK_FLUSH);  // stream order: the next launch sees these deltas applied; nothing to wait for
+    ctl.seq++;
     ctl.n_delta = 0;
   }
 
-  // actions/allocate/allocate.go:46-111 — same steps as sequencer_main of the device-resident mode
+  // actions/allocate/allocate.go:46-111
   void run_allocate() {
     const DevSnap &s = *seq.s;
     double t_begin = now();
@@ -790,6 +683,6 @@ struct HostBackend {
   }
 };
 
-inline void host_flush_deltas(Seq &q) { ((HostBackend *)q.host_backend)->flush_deltas(); }
+void seq_flush_deltas(Seq &q) { ((HostBackend *)q.host_backend)->flush_deltas(); }
 
 }  // namespace kai

@@ -4,9 +4,8 @@
 //   k_queue_usage    per-queue Allocated / Request scatter-add    (proportion.go:347-401)  } oracle's order
 //   k_queue_usage_ordered  the oracle's order where k_queue_usage's sums could round      } (DESIGN.md §2)
 //   k_fair_share     hierarchical fair-share division per level   (resource_division.go:26-357)
-//   k_action         persistent cooperative kernel running a whole Action (allocate) on device:
-//                    node tiles resident in shared memory, one fit+score+argmax sweep per
-//                    allocateTask, one all-to-all slot exchange per sweep, replicated sequencer.
+//
+// The sweep kernels of an action are in kai_action.cuh.
 //
 // All arithmetic that feeds a decision is IEEE binary64 with explicit round-to-nearest
 // intrinsics (no FMA contraction; the file is also compiled with -fmad=false) in the
@@ -16,7 +15,6 @@
 #include <cstdint>
 
 #include "kai_device.cuh"
-#include "kai_seq.cuh"
 
 namespace kai {
 

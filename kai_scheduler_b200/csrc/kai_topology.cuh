@@ -628,7 +628,7 @@ struct TopologyHost {
     gpu_set.clear();
     gpu_pref_level = -1;
   }
-  void reset_gpu_state() {  // a new k_action launch starts with scoring off and an undefined table
+  void reset_gpu_state() {  // a new action starts with scoring off and an undefined table
     gpu_pref_level = -1;
     gpu_set.clear();
     if (!gpu_bucket.empty()) std::fill(gpu_bucket.begin(), gpu_bucket.end(), 255);

@@ -60,7 +60,6 @@ int main() {
   hb.seq.ctl = &hb.ctl;
   hb.seq.delta_base = delta_buf.data();
   hb.seq.host_backend = &hb;
-  hb.launch_mode = true;
   hb.launch_fn = &fake_launch;
   hb.rank_to_node = rank_to_node.data();
   hb.ctl.seq = 7;
@@ -182,7 +181,7 @@ int main() {
     CHECK(hb.list_valid == valid, "trial %d (S=%d): valid prefix %zu, want %zu", trial, S, hb.list_valid, valid);
     CHECK(hb.list_more == have_cut, "trial %d: more flag", trial);
     for (size_t i = 0; i < valid; i++)
-      CHECK(hb.list[i].score == all[i].score && hb.list[i].rank == all[i].rank && hb.list[i].cap == 3 && hb.list[i].loaded &&
+      CHECK(hb.list[i].score == all[i].score && hb.list[i].rank == all[i].rank && hb.list[i].cap == 3 &&
                 hb.list[i].node == (int)all[i].rank,
             "trial %d entry %zu", trial, i);
     CHECK(hb.ctl.seq == seq_no + 1 && hb.ctl.n_delta == 0, "trial %d: sequence", trial);

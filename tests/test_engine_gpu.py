@@ -189,14 +189,11 @@ def test_solver_tables_forced_grid(grid, env, monkeypatch):
         assert_same(re_, ro)
 
 
-@pytest.mark.parametrize("grid,mode", [("2", "host"), ("3", "device"), ("148", "host"), ("148", "device")])
-def test_allocate_tables_forced_grid(grid, mode, monkeypatch):
-    """Same tables with forced CTA counts (including scanners that own no node), both sequencer modes."""
+@pytest.mark.parametrize("grid", ["2", "3", "148"])
+def test_allocate_tables_forced_grid(grid, monkeypatch):
+    """Same tables with forced CTA counts (including scanners that own no node)."""
     monkeypatch.setenv("KAI_GRID_EXACT", grid)
-    monkeypatch.setenv("KAI_SEQUENCER", mode)
     for cid, case in ALLOCATE:
-        if mode == "device" and case["topology"].get("Topologies"):
-            continue  # topology constraints run host-sequenced only
         snap, meta = dsl.build_snapshot(case["topology"])
         re_, ro = run_both(snap, cfg=case_config(case))
         assert_same(re_, ro)
@@ -215,11 +212,9 @@ def test_synthetic_parity(kw):
     assert_same(re_, ro)
 
 
-@pytest.mark.parametrize("env", [("KAI_NO_BATCHING", "1"), ("KAI_NO_TOPM", "1"), ("KAI_NO_SMEM_HOT", "1"),
-                                 ("KAI_SEQUENCER", "device")])
+@pytest.mark.parametrize("env", [("KAI_NO_BATCHING", "1"), ("KAI_NO_TOPM", "1")])
 def test_synthetic_parity_fallback_paths(env, monkeypatch):
-    """Same answers with batching off, with single-candidate answers (no top-M lists), with the sequencer's hot arrays
-    in global memory, and with the device-resident sequencer (CTA 0) instead of the host-sequenced default."""
+    """Same answers with batching off, and with single-candidate answers (no top-M lists)."""
     monkeypatch.setenv(env[0], env[1])
     for kw in (dict(n_nodes=300, n_jobs=400, tasks_per_job=4, n_queues=12),
                dict(n_nodes=257, n_jobs=600, tasks_per_job=3, n_queues=7, mixed=True)):
@@ -350,12 +345,10 @@ def test_historical_usage_and_k_value(k_value):
     assert not np.array_equal(plain.run("allocate").queue_fair_share, ro.queue_fair_share)  # usage is not vacuous
 
 
-@pytest.mark.parametrize("grid", [None, "5"])
-def test_tables_persistent_transport(grid, monkeypatch):
-    """The cooperative scan-server kernel (KAI_TRANSPORT=persistent; the default transport is one launch per record)."""
-    monkeypatch.setenv("KAI_TRANSPORT", "persistent")
-    if grid:
-        monkeypatch.setenv("KAI_GRID_EXACT", grid)
+def test_tables_grid5_top_m_lists(monkeypatch):
+    """Four scanners (not a power of two) with top-M lists on: the allocate and solver tables, a mixed 1 000-node
+    snapshot and config4-small."""
+    monkeypatch.setenv("KAI_GRID_EXACT", "5")
     for cid, case in ALLOCATE:
         snap, meta = dsl.build_snapshot(case["topology"])
         re_, ro = run_both(snap, cfg=case_config(case))
@@ -367,6 +360,29 @@ def test_tables_persistent_transport(grid, monkeypatch):
     snap = synthetic.benchmark_snapshot(n_nodes=1000, n_jobs=3000, tasks_per_job=2, n_queues=40, mixed=True)
     assert_same(*run_both(snap))
     snap = synthetic.config_snapshot("config4-small")
+    assert_same(*run_both(snap))
+
+
+@pytest.mark.parametrize("env", [("KAI_TRANSPORT", "persistent"), ("KAI_SEQUENCER", "device")])
+def test_removed_modes_are_refused(env, monkeypatch):
+    """The persistent transport and the device-resident sequencer no longer exist: selecting one fails the action
+    with KAI_ERR_UNSUPPORTED and names the variable, instead of running the default path under the old name."""
+    from kai_scheduler_b200.engine import EngineError
+    snap = synthetic.benchmark_snapshot(n_nodes=16, n_jobs=20, tasks_per_job=1, n_queues=2)
+    e = Engine()
+    e.load(snap)
+    monkeypatch.setenv(*env)
+    with pytest.raises(EngineError, match=f"{env[0]}={env[1]}"):
+        e.run("allocate")
+    monkeypatch.delenv(env[0])
+    assert_same(e.run("allocate"), run_both(snap)[1])
+    e.close()
+
+
+def test_300k_nodes_small_allocate():
+    """300 000 nodes on one GPU: 256 scanners of ~1 172 rows, whose tiles fit k_record's shared memory.  A few hundred
+    pods against the oracle."""
+    snap = synthetic.benchmark_snapshot(n_nodes=300_000, n_jobs=300, tasks_per_job=2, n_queues=8, mixed=True)
     assert_same(*run_both(snap))
 
 

@@ -150,8 +150,6 @@ def test_resident_cycles_synthetic(kind, kw):
 
 
 PATHS = [
-    ("persistent", {"KAI_TRANSPORT": "persistent"}, ACTIONS),
-    ("device-sequencer", {"KAI_SEQUENCER": "device"}, ["allocate"]),
     ("grid2", {"KAI_GRID_EXACT": "2"}, ACTIONS),
     ("grid5", {"KAI_GRID_EXACT": "5"}, ACTIONS),
     ("no-topm", {"KAI_NO_TOPM": "1"}, ACTIONS),
@@ -160,7 +158,7 @@ PATHS = [
 
 @pytest.mark.parametrize("name,env,actions", PATHS, ids=[p[0] for p in PATHS])
 def test_resident_cycles_every_path(monkeypatch, name, env, actions):
-    """The fuzz subset through the other transports, sequencer and forced grids."""
+    """The fuzz subset through forced grids and single-candidate answers."""
     for k, v in env.items():
         monkeypatch.setenv(k, v)
     for seed in range(30):

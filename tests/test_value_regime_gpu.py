@@ -3,8 +3,7 @@
 Every regime runs allocate, consolidation, reclaim, preempt and stalegangeviction on one session and compares every
 table of every action with the oracle, the fair shares included (k_fair_share uses the oracle's operations: no
 tolerance).  The same runs repeat on two fresh engines and a resident reload (the bits must not change from run to
-run), under forced grids, the persistent transport, the device sequencer, single-candidate answers and without the
-fresh-gang bulk path.  test_value_regime.py shows on the CPU that each regime reaches the case it targets.
+run), under forced grids, with single-candidate answers and without the fresh-gang bulk path.  test_value_regime.py shows on the CPU that each regime reaches the case it targets.
 """
 import functools
 
@@ -65,8 +64,7 @@ def test_regime_runs_are_deterministic(name):
     e2.close()
 
 
-KNOBS = [("KAI_GRID_EXACT", "2"), ("KAI_GRID_EXACT", "5"), ("KAI_TRANSPORT", "persistent"), ("KAI_SEQUENCER", "device"),
-         ("KAI_NO_TOPM", "1"), ("KAI_NO_GANG_FAST", "1")]
+KNOBS = [("KAI_GRID_EXACT", "2"), ("KAI_GRID_EXACT", "5"), ("KAI_NO_TOPM", "1"), ("KAI_NO_GANG_FAST", "1")]
 
 
 @pytest.mark.parametrize("knob", KNOBS, ids=[f"{k}={v}" for k, v in KNOBS])
@@ -81,12 +79,7 @@ def test_regime_paths(name, knob, monkeypatch):
             e.load(snap)
         e.close()
         return
-    if knob[0] == "KAI_SEQUENCER":  # the device-resident sequencer runs allocate only
-        res_e, res_o = _engine_cycle(e, snap, ("allocate",)), _oracle_cycle(name)[:1]
-        assert_same(res_e[0], res_o[0])
-        np.testing.assert_array_equal(res_e[0].queue_fair_share, res_o[0].queue_fair_share)
-    else:
-        _check(_engine_cycle(e, snap), _oracle_cycle(name))
+    _check(_engine_cycle(e, snap), _oracle_cycle(name))
     e.close()
 
 
