@@ -1298,8 +1298,9 @@ __device__ void reduce_answers(const ActionParams &p, int kind, unsigned int seq
 // =============================================================================================
 // list answers: merge of the scanners' top-M candidates
 // =============================================================================================
-// Integer sort keys of a candidate: h = ~bits(score) (scores are sums of non-negative terms, so ascending h is descending
-// score), l = rank << 32 | source (scanner * kTopM + m); an empty slot is all ones in both and sorts last.
+// Integer sort keys of a candidate: h = list_key(score) (ascending h is descending score for any non-NaN score: DK_TOPK
+// scores, Idle + Releasing GPUs, go negative on over-committed nodes; -0.0 and +0.0 share a key), l = rank << 32 |
+// source (scanner * kTopM + m); an empty slot is all ones in both and sorts last.
 constexpr int kMergeThreads = 1024;  // one candidate per thread: scanners x kTopM <= 1024
 __device__ __forceinline__ bool mk_before(unsigned long long ah, unsigned long long al, unsigned long long bh, unsigned long long bl) {
   return ah < bh || (ah == bh && al < bl);
@@ -1347,7 +1348,7 @@ __global__ void __cluster_dims__(kMergeCtas, 1, 1) __launch_bounds__(kMergeCtaTh
     const uint32_t rank = (uint32_t)(hi & 0xffffffu);
     more = (((uint32_t)(hi >> 32) & 0xffu) & LF_MORE) != 0;
     if (rank != kRankNone) {
-      h = ~lo;
+      h = list_key(__longlong_as_double((long long)lo));
       l = ((unsigned long long)rank << 32) | (unsigned long long)g;
     }
   }

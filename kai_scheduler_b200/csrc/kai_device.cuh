@@ -76,6 +76,15 @@ KAI_HD inline unsigned long long kbits(double x) {
   memcpy(&u, &x, 8);
   return u;
 }
+// Sort key of a list candidate's score: ascending key = descending score for every non-NaN double, negatives and
+// +-inf included, and -0.0 gets the key of +0.0 (they compare equal, so the name rank decides between them).  Negative
+// scores keep their bits (a larger magnitude sorts later); non-negative ones flip the 63 value bits, which keeps their
+// relative order and clears the top bit.  Every key is at most 0xfff0000000000000 (-inf), below ~0ull (an empty slot).
+KAI_HD inline unsigned long long list_key(double x) {
+  unsigned long long u = kbits(x);
+  if (u == 0x8000000000000000ull) u = 0;  // -0.0
+  return (u >> 63) ? u : u ^ 0x7fffffffffffffffull;
+}
 KAI_HD inline double requestable_share(double max_allowed, double request) {
   if (max_allowed == KAI_UNLIMITED) return request;
   return fmin(max_allowed, request);

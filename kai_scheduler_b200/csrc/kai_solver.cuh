@@ -753,27 +753,57 @@ struct Solver {
   // the k rows with most idle + releasing GPUs (values, descending); pages of top-M lists until k are known
   std::vector<std::pair<double, int>> sweep_topk_idle(int k, unsigned int snap_bits) {
     std::vector<std::pair<double, int>> host;
-    if (host_sweep_max > 0 && host_topk(k, host)) {
-      if (!host_sweep_check) {
-        if (snap_bits) {  // the feasible-set snapshot still reaches the scanners, without a round trip
-          ctl.xbits = snap_bits;
-          hb.flush_deltas();
-          ctl.xbits = 0;
-        }
-        host_topks++;
-        return host;
-      }
-      std::vector<std::pair<double, int>> dev = sweep_topk_idle_gpu(k, snap_bits);
-      if (!hb.failed && dev != host) {
-        snprintf(hb.error_msg, sizeof(hb.error_msg),
-                 "KAI_HOST_SWEEP_CHECK: top-%d idle-GPU rows differ: host %zu rows (first node %d), GPU %zu rows (first node %d)",
-                 k, host.size(), host.empty() ? -1 : host[0].second, dev.size(), dev.empty() ? -1 : dev[0].second);
-        seq.error = kSeqErrHostSweep;
+    const bool on_host = host_sweep_max > 0 && host_topk(k, host);
+    if (on_host && !host_sweep_check) {
+      if (snap_bits) {  // the feasible-set snapshot still reaches the scanners, without a round trip
+        ctl.xbits = snap_bits;
+        hb.flush_deltas();
+        ctl.xbits = 0;
       }
       host_topks++;
       return host;
     }
-    return sweep_topk_idle_gpu(k, snap_bits);
+    std::vector<std::pair<double, int>> dev = sweep_topk_idle_gpu(k, snap_bits);
+    // KAI_HOST_SWEEP_CHECK: every answer, the GPU's list and the host one, against the plain restatement over all rows
+    // (one GPU: a shard's mirror holds every row, but its list only its own)
+    if (host_sweep_check && seq.mirror && cfg.shard_count <= 1 && !hb.failed) {
+      const std::vector<std::pair<double, int>> ref = topk_reference(k);
+      if (on_host) topk_check("host", k, host, ref);
+      topk_check("GPU", k, dev, ref);
+    }
+    if (on_host) {
+      host_topks++;
+      return host;
+    }
+    return dev;
+  }
+  // The k rows with most idle + releasing GPUs, restated: every mirror row, key = Idle + Releasing GPUs, sorted by key
+  // descending and name rank ascending (-0.0 == +0.0, so the rank decides between them).
+  std::vector<std::pair<double, int>> topk_reference(int k) const {
+    std::vector<int> rows(N);
+    for (int n = 0; n < N; n++) rows[n] = n;
+    const size_t m = std::min((size_t)std::max(k, 0), (size_t)N);
+    auto key = [&](int n) { return kadd(Ig(n), Lg(n)); };
+    std::partial_sort(rows.begin(), rows.begin() + m, rows.end(), [&](int a, int b) {
+      const double ka = key(a), kb = key(b);
+      return ka > kb || (ka == kb && s.name_rank[a] < s.name_rank[b]);
+    });
+    std::vector<std::pair<double, int>> out;
+    for (size_t i = 0; i < m; i++) out.push_back({key(rows[i]), rows[i]});
+    return out;
+  }
+  void topk_check(const char *who, int k, const std::vector<std::pair<double, int>> &got,
+                  const std::vector<std::pair<double, int>> &ref) {
+    if (seq.error == kSeqErrHostSweep) return;  // the first difference is the one reported
+    size_t i = 0;
+    while (i < got.size() && i < ref.size() && got[i] == ref[i]) i++;  // pair ==: values compare as doubles
+    if (i == got.size() && i == ref.size()) return;
+    snprintf(hb.error_msg, sizeof(hb.error_msg),
+             "KAI_HOST_SWEEP_CHECK: top-%d idle-GPU rows differ: %s %zu rows, reference %zu rows; first difference at "
+             "%zu: %s node %d (%g), reference node %d (%g)",
+             k, who, got.size(), ref.size(), i, who, i < got.size() ? got[i].second : -1, i < got.size() ? got[i].first : 0.0,
+             i < ref.size() ? ref[i].second : -1, i < ref.size() ? ref[i].first : 0.0);
+    seq.error = kSeqErrHostSweep;
   }
   // The same k rows from the mirror: every row with idle + releasing GPUs > 0 is in gpu_free_list; after them come the
   // rows whose sum is exactly 0, in name-rank order (rows below 0 would follow: the GPU answers when they are needed).

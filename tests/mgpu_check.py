@@ -50,10 +50,14 @@ def main():
         print(f"rank {rank}/{world} {kw}: {'OK' if same else 'MISMATCH'} placed {res.pods_placed} sweeps {eng.stats().decisions}",
               flush=True)
         ok = ok and same
-    # one whole cycle (allocate, consolidation, reclaim, preempt, stalegangeviction) on node-striped GPUs
-    for kw in (dict(n_nodes=48, running_per_node=7, victim_queues=2, reclaimer_jobs=12, reclaimer_tasks=2, reclaimer_gpus=3.0),
-               dict(n_nodes=100), dict(n_nodes=333, running_per_node=8, victim_queues=3, reclaimer_jobs=9, reclaimer_tasks=3, reclaimer_gpus=4.0)):
-        snap = synthetic.reclaim_snapshot(**kw)
+    # one whole cycle (allocate, consolidation, reclaim, preempt, stalegangeviction) on node-striped GPUs; the last
+    # cluster has over-committed GPU nodes (negative idle GPUs): every rank's merged top-k list is cut at a negative key
+    import value_regime as vr
+    cycles = [(kw, synthetic.reclaim_snapshot(**kw)) for kw in (
+        dict(n_nodes=48, running_per_node=7, victim_queues=2, reclaimer_jobs=12, reclaimer_tasks=2, reclaimer_gpus=3.0),
+        dict(n_nodes=100), dict(n_nodes=333, running_per_node=8, victim_queues=3, reclaimer_jobs=9, reclaimer_tasks=3, reclaimer_gpus=4.0))]
+    cycles.append(("overcommitted_gpus(333)", vr.overcommitted_gpus(333, 6, (1, 2, 3, 4, 8), stripes=(1, 3))))
+    for kw, snap in cycles:
         eng.load(snap)
         o = Oracle()
         o.load(snap)
@@ -68,7 +72,6 @@ def main():
             print(f"rank {rank}/{world} cycle {kw} {action}: {'OK' if same else 'MISMATCH'} placed {res.pods_placed} evicted {res.pods_evicted}", flush=True)
             ok = ok and same
     # non-round values (tests/value_regime.py): inexact node totals and queue sums must give every rank the oracle's bits
-    import value_regime as vr
     for name in ("a_totals", "b_queues"):
         snap, _ = vr.regime(name)  # both regimes run with the default configuration
         eng.load(snap)

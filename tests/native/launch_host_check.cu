@@ -1,8 +1,11 @@
 // Host-only check of the launch transport's host side (kai_host_seq.cuh): (1) a decision record is packed into the
 // LaunchRec a k_record launch carries exactly as the scanners decode it (folded node deltas, repeat counts, extended
-// entries), (2) the merged candidate lists of several GPUs are merged with the cut rule applied across ranks.
+// entries), (2) the merged candidate lists of several GPUs are merged with the cut rule applied across ranks, negative
+// and -0.0 scores included, (3) the integer sort key of k_merge_cluster orders every score as the comparator does.
 // Built and run by tests/test_launch_host.py (nvcc, no GPU needed: nothing is launched).
 #include <algorithm>
+#include <cfloat>
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -148,7 +151,9 @@ int main() {
     for (int r = 0; r < S; r++) {
       const int n = (int)(rnd() % 40);
       std::vector<Ent> mine;
-      for (int i = 0; i < n; i++) mine.push_back({(double)(rnd() % 5), ranks[next_rank++]});  // few score levels: many ties
+      // few score levels, many ties; negative idle GPUs (over-committed nodes) and -0.0 (== +0.0: the rank decides)
+      static const double levels[] = {4.0, 2.0, 1.0, 0.0, -0.0, -1.0, -3.0};
+      for (int i = 0; i < n; i++) mine.push_back({levels[rnd() % 7], ranks[next_rank++]});
       std::sort(mine.begin(), mine.end(), before);
       const bool more = (rnd() & 1) != 0;
       unsigned long long *cl = clist.data() + ((size_t)r * 2 + (seq_no & 1)) * kCListWords;
@@ -186,6 +191,69 @@ int main() {
             "trial %d entry %zu", trial, i);
     CHECK(hb.ctl.seq == seq_no + 1 && hb.ctl.n_delta == 0, "trial %d: sequence", trial);
   }
-  printf("OK record packing (%zu deltas, flush) and 200 multi-GPU list merges\n", want.size());
+
+  // ---------------------------------------------------------------- (3) the list merge's sort key
+  // k_merge_cluster sorts candidates by (list_key(score), rank << 32 | source) as unsigned integers; that order must be
+  // the comparator's (score desc, rank asc) for every score a list can carry, and every real key must precede the
+  // empty slot (~0ull).
+  {
+    auto dbl = [](unsigned long long u) {
+      double d;
+      memcpy(&d, &u, 8);
+      return d;
+    };
+    const double specials[] = {0.0, -0.0, 1.0, -1.0, 8.0, -3.0, 0.5, -0.5, DBL_MAX, -DBL_MAX, DBL_MIN, -DBL_MIN,
+                               dbl(1), dbl(0x8000000000000001ull), dbl(0x000fffffffffffffull), dbl(0x800fffffffffffffull),
+                               HUGE_VAL, -HUGE_VAL, 1e300, -1e300, 2.0 - 1e-15, 2.0 + 4e-16};
+    const int n_spec = (int)(sizeof(specials) / sizeof(specials[0]));
+    for (int v = 0; v < n_spec; v++)
+      CHECK(list_key(specials[v]) < ~0ull, "key of %a reaches the empty slot", specials[v]);
+    CHECK(list_key(0.0) == list_key(-0.0), "-0.0 and +0.0 keys differ");
+    CHECK(list_key(2.0) == ~kbits(2.0) - (1ull << 63), "non-negative keys keep their order: ~bits with the top bit cleared");
+    long long pairs = 0;
+    for (int trial = 0; trial < 300; trial++) {
+      const int n = 1 + (int)(rnd() % 600);
+      struct C {
+        double v;
+        unsigned int rank, src;
+      };
+      std::vector<C> c(n);
+      std::vector<unsigned int> rk(n);
+      for (int i = 0; i < n; i++) rk[i] = (unsigned int)i;
+      for (int i = n - 1; i > 0; i--) std::swap(rk[i], rk[rnd() % (i + 1)]);
+      for (int i = 0; i < n; i++) {
+        double v;
+        switch (rnd() % 6) {
+          case 0: v = specials[rnd() % n_spec]; break;
+          case 1: v = (double)((int)(rnd() % 9) - 4); break;  // exact ties around 0
+          case 2: v = (rnd() & 1) ? 0.0 : -0.0; break;
+          case 3: v = dbl(((unsigned long long)rnd() << 32 | rnd()) & 0x800fffffffffffffull); break;  // subnormal
+          case 4: v = ((double)rnd() - 2147483648.0) * 1e-3; break;
+          default: {  // any finite bit pattern
+            unsigned long long u;
+            do u = (unsigned long long)rnd() << 32 | rnd();
+            while (((u >> 52) & 0x7ff) == 0x7ff);
+            v = dbl(u);
+          }
+        }
+        c[i] = {v, rk[i], (unsigned int)i};
+      }
+      std::vector<int> want_p(n), got_p(n);
+      for (int i = 0; i < n; i++) want_p[i] = got_p[i] = i;
+      std::sort(want_p.begin(), want_p.end(), [&](int a, int b) { return c[a].v > c[b].v || (c[a].v == c[b].v && c[a].rank < c[b].rank); });
+      std::sort(got_p.begin(), got_p.end(), [&](int a, int b) {
+        const unsigned long long ha = list_key(c[a].v), hb_ = list_key(c[b].v);
+        const unsigned long long la = (unsigned long long)c[a].rank << 32 | c[a].src, lb = (unsigned long long)c[b].rank << 32 | c[b].src;
+        return ha < hb_ || (ha == hb_ && la < lb);
+      });
+      for (int i = 0; i < n; i++)
+        CHECK(want_p[i] == got_p[i], "key trial %d: position %d holds %a (rank %u), want %a (rank %u)", trial, i, c[got_p[i]].v,
+              c[got_p[i]].rank, c[want_p[i]].v, c[want_p[i]].rank);
+      for (int i = 0; i < n; i++) CHECK(list_key(c[i].v) < ~0ull, "key trial %d: %a reaches the empty slot", trial, c[i].v);
+      pairs += n;
+    }
+    printf("OK record packing (%zu deltas, flush), 200 multi-GPU list merges and the list sort key (%lld candidates)\n",
+           want.size(), pairs);
+  }
   return 0;
 }

@@ -114,13 +114,70 @@ def test_d_fair_shares_take_the_fractional_paths():
 
 
 def test_regimes_keep_node_accounting_consistent():
-    """Idle + Releasing + the active pods' requests + the foreign pods = Allocatable on every node."""
+    """Idle + the placed pods' requests (Pipelined ones aside) + the foreign pods = Allocatable on every node, and
+    Releasing = the Releasing pods' requests - the Pipelined pods' requests.  Only the over-committed regimes (e) have
+    nodes with negative Idle."""
     for name in vr.REGIMES:
         snap, _ = vr.regime(name)
         used = np.zeros_like(snap.node_allocatable)
+        rel = np.zeros_like(snap.node_allocatable)
         for t in np.flatnonzero(snap.task_node >= 0):
-            used[:, snap.task_node[t]] += snap.task_req[t]
+            n, st = snap.task_node[t], snap.task_status[t]
+            if st == abi.POD_PIPELINED:
+                rel[:, n] -= snap.task_req[t]
+                continue
+            used[:, n] += snap.task_req[t]
+            if st == abi.POD_RELEASING:
+                rel[:, n] += snap.task_req[t]
         if snap.node_foreign is not None:
             used[:3] += snap.node_foreign
-        np.testing.assert_array_equal(snap.node_idle + snap.node_releasing + used - snap.node_allocatable, 0, err_msg=name)
-        assert (snap.node_idle[:3] >= 0).all(), name
+        np.testing.assert_array_equal(snap.node_idle + used - snap.node_allocatable, 0, err_msg=name)
+        np.testing.assert_array_equal(snap.node_releasing - rel, 0, err_msg=name)
+        if not name.startswith("e_"):
+            assert (snap.node_idle[:3] >= 0).all(), name
+
+
+E_REGIMES = [n for n in vr.REGIMES if n.startswith("e_")]
+
+
+@pytest.mark.parametrize("name", E_REGIMES)
+def test_e_overcommitted_rows_reach_the_negative_list_keys(name):
+    """The over-committed regimes put negative idle-GPU keys where the top-k list's sort and cut meet them."""
+    snap, cfg = vr.regime(name)
+    G, N = abi.RES_GPU, snap.n_nodes
+    idle, rel, alloc = snap.node_idle[G], snap.node_releasing[G], snap.node_allocatable[G]
+    key = vr.idle_gpu_key(snap)
+    assert (idle < 0).sum() >= N // 4 and set(np.unique(idle[(idle < 0) & (alloc > 0)])) >= {-1.0, -2.0, -3.0}
+    assert ((idle < 0) & (rel > 0)).any()                       # Releasing pod on an over-committed node
+    assert (rel < 0).any()                                      # Pipelined pod
+    assert ((alloc == 0) & (idle < 0)).sum() == 2               # binpack's overall == 0 skip with pods running
+    assert ((alloc != 0) & (idle < 0)).any()                    # binpack's minimum is negative
+    mz = (key == 0) & np.signbit(key)
+    assert mz.sum() >= 3 and np.signbit(idle[mz]).all() and np.signbit(rel[mz]).all()
+    pz = np.flatnonzero((key == 0) & ~np.signbit(key))
+    assert len(pz) > 0 and snap.node_name_rank[pz].min() < snap.node_name_rank[mz].max()   # -0.0 and +0.0 ranks interleave
+    # the page-and-cut loop meets a negative cut: with 4 scanners (KAI_GRID_EXACT=5) and, where a scanner of the default
+    # grid (min(256, N) scanners) holds >= 5 rows, there too
+    assert vr.stripe_cut_goes_negative(snap, 4)
+    if N // min(256, N) >= 5:
+        assert vr.stripe_cut_goes_negative(snap, min(256, N))
+    # the filter needs more rows than have a key >= 0 (e_overcommit), or more than 256 rows have free GPUs, which is
+    # past the host answer's default limit (e_overcommit_2048)
+    gangs = np.diff(snap.podset_task_begin)[snap.task_status[snap.podset_task_begin[:-1]] == abi.POD_PENDING]
+    if name == "e_overcommit":
+        assert gangs.max() > (key >= 0).sum()
+    else:
+        assert (key > 0).sum() > 256
+
+
+@pytest.mark.parametrize("name,action", [("e_overcommit", "reclaim"), ("e_overcommit_2048", "consolidation"),
+                                         ("e_overcommit_2048", "reclaim")])
+def test_e_workloads_evict(name, action):
+    """The oracle's reclaim and consolidation evict pods on these clusters: the engine's victims are compared, not an
+    empty answer."""
+    snap, cfg = vr.regime(name)
+    o = Oracle(cfg)
+    o.load(snap)
+    res = o.run(action)
+    o.close()
+    assert res.pods_evicted > 0

@@ -73,8 +73,9 @@ def test_regime_paths(name, knob, monkeypatch):
     monkeypatch.setenv(*knob)
     snap, cfg = vr.regime(name)
     e = Engine(cfg)
-    if knob == ("KAI_GRID_EXACT", "2") and snap.n_nodes >= 5000:
-        # one scanner CTA would have to hold every node row in shared memory: the engine refuses instead of guessing
+    if knob == ("KAI_GRID_EXACT", "2") and snap.n_nodes >= 2048:
+        # one scanner CTA would have to hold every node row in shared memory (100 B a row with 4 resources, 227 KB of
+        # shared memory per CTA on an H100, 40 KB of it kept for k_record): the engine refuses instead of guessing
         with pytest.raises(EngineError, match="node tile does not fit"):
             e.load(snap)
         e.close()

@@ -4,7 +4,8 @@ The synthetic and DSL clusters use round quantities (2e7 mCPU / 2e10 B nodes, 10
 On such data every f64 sum on the scheduling path is exact, so it has the same bits in any order and association, and
 a kernel that sums in another order than the oracle (DESIGN.md §2) or reassociates a formula still matches.  The
 generators here keep the structure of those shapes and rewrite their values into realistic, non-round Kubernetes
-quantities (arbitrary milli-CPU, memory in Ki multiples, odd byte counts), in four regimes:
+quantities (arbitrary milli-CPU, memory in Ki multiples, odd byte counts), in four regimes, plus (e) with negative
+Idle GPUs:
 
   (a) inexact_totals      >= 5 000 ~2 TB nodes, each with a foreign pod of an odd byte count: the memory total passes
                           2^53 at a granularity of 1 B, so the order of the node sum decides its bits.
@@ -14,6 +15,8 @@ quantities (arbitrary milli-CPU, memory in Ki multiples, odd byte counts), in fo
                           larger node: binpack / spread scores differ in the last bits or tie (the name rank decides);
                           plus the edges mn == mx, mx == 0 and overall == 0.
   (d) fractional_shares   non-integer k_value, historical usage, over-quota weights, deserved quotas and CPU totals.
+  (e) overcommitted_gpus  nodes whose running pods hold more GPUs than the node has: negative Idle GPUs, which the
+                          idle-GPU filter's top-k list must order below zero (and -0.0 rows equal to +0.0 ones).
 
 It also holds the exact references the CPU tests use: Fraction sums, the sequential rounding bound, a numpy emulation
 of k_node_totals' reduction order, and a restatement of SetResourcesShare that reports which paths it took.
@@ -174,8 +177,72 @@ def fractional_shares(seed: int = 5):
     return refresh_node_tables(snap), 0.37
 
 
+def _trim_gangs(snap: abi.Snapshot, n_run: int, sizes) -> abi.Snapshot:
+    """Cuts reclaim_snapshot's equal reclaimer gangs (jobs after the n_run 1-task victims) to `sizes` tasks each."""
+    top = int(max(sizes))
+    keep = np.ones(snap.n_tasks, dtype=bool)
+    for g, size in enumerate(sizes):
+        keep[n_run + g * top + size:n_run + (g + 1) * top] = False
+    snap.task_status, snap.task_node = snap.task_status[keep], snap.task_node[keep]
+    snap.task_req = snap.task_req[keep]
+    snap.task_order_rank = np.concatenate(
+        [snap.task_order_rank[:n_run]] + [synthetic._name_rank("", size) for size in sizes]).astype(np.int32)
+    snap.podset_min_available = np.concatenate([np.ones(n_run), np.asarray(sizes)]).astype(np.int32)
+    snap.podset_task_begin = np.concatenate([np.arange(n_run), n_run + np.cumsum([0] + list(sizes))]).astype(np.int32)
+    return snap
+
+
+def overcommitted_gpus(n_nodes: int, running_per_node: int, gang_sizes, stripes=(1,), preemptible_every: int = 1,
+                       seed: int = 7) -> abi.Snapshot:
+    """(e) Over-committed GPU nodes: nodes whose GPU allocatable fell below the GPUs their running pods hold (a
+    device-plugin restart or a GPU marked unhealthy), so Idle GPUs = -1..-3 (node_info.go addTask subtracts without a fit
+    check and nothing clamps it).  Base: reclaim_snapshot with `running_per_node` running 1-GPU pods per node in two
+    victim queues (deserved 0) and pending gangs of `gang_sizes` 8-GPU tasks in the reclaimer queue; the running pods
+    are preemptible on every `preemptible_every`-th node only (fewer candidate victims keep the oracle's search short).
+
+    Over-committed: every node of the name-rank stripes rank % 4 in `stripes` but the first three of each (a scanner of
+    a 4- or 256-scanner grid holds ranks j * nscan + my, so its 4th candidate is negative and it has more rows), plus
+    one node in 24 elsewhere.  Edge rows: a Releasing pod on an over-committed node (Idle < 0, Releasing > 0), a
+    Pipelined pod (Releasing < 0), two nodes with no GPU allocatable and pods still running, and ten full nodes in
+    interleaved name ranks, five with Idle and Releasing GPUs +0.0 and five with -0.0.  Three nodes are empty: no gang
+    fits on them alone, but they count in the filter's top-k, so a list that drops them prunes scenarios the oracle
+    simulates."""
+    rng = np.random.default_rng(seed)
+    snap = synthetic.reclaim_snapshot(n_nodes, running_per_node=running_per_node, victim_queues=2,
+                                      reclaimer_jobs=len(gang_sizes), reclaimer_tasks=int(max(gang_sizes)), reclaimer_gpus=8.0)
+    N, n_run, G = n_nodes, n_nodes * running_per_node, abi.RES_GPU
+    snap = _trim_gangs(snap, n_run, gang_sizes)
+    snap.job_flags[:n_run][snap.task_node[:n_run] % preemptible_every != 0] &= ~np.uint32(abi.JOB_PREEMPTIBLE)
+    rank_to_node = np.argsort(snap.node_name_rank)
+    over = np.zeros(N, dtype=bool)
+    for st in stripes:
+        over[rank_to_node[st + 4 * 3::4]] = True
+    free = np.flatnonzero(~over)
+    over[rng.choice(free, size=max(1, N // 24), replace=False)] = True
+    snap.node_allocatable[G, over] = running_per_node - rng.integers(1, 4, size=int(over.sum()))
+    rest = rank_to_node[[r for r in range(N) if not over[rank_to_node[r]]]]   # not over-committed, in name-rank order
+    zero_alloc, minus_zero, plus_zero = rest[[3, len(rest) // 2]], rest[[5, 9, 13, 17, 21]], rest[[7, 11, 15, 19, 23]]
+    snap.node_allocatable[G, zero_alloc] = 0.0
+    snap.node_allocatable[G, np.concatenate([minus_zero, plus_zero])] = running_per_node
+    free = rest[[27, len(rest) // 3, 2 * len(rest) // 3 + 1]]   # every pod on them finished: Idle = 8
+    done = np.flatnonzero(np.isin(snap.task_node[:n_run], free))
+    snap.task_status[done] = abi.POD_STATUS_NAMES["Succeeded"]
+    snap.task_node[done] = -1
+    on_over = np.flatnonzero(over[snap.task_node[:n_run]])
+    snap.task_status[on_over[0]] = abi.POD_RELEASING
+    snap.task_status[on_over[-1]] = abi.POD_PIPELINED
+    snap = refresh_node_tables(snap)
+    snap.node_idle[G, minus_zero] = -0.0
+    snap.node_releasing[G, minus_zero] = -0.0
+    return snap
+
+
 def regime(name: str):
     """(snapshot, config) of a named regime."""
+    if name == "e_overcommit":  # one row per scanner of the default grid; the largest gang needs more rows than are >= 0
+        return overcommitted_gpus(96, 6, (4, 5, 6, 50), stripes=(1, 3)), abi.make_config()
+    if name == "e_overcommit_2048":  # > 256 rows with free GPUs: even the default mode lists them on the GPU
+        return overcommitted_gpus(2048, 6, (4, 5, 6, 8), preemptible_every=8), abi.make_config()
     if name == "a_totals":
         return inexact_totals(), abi.make_config()
     if name == "a_totals_1800":  # fits one node tile of a 2-CTA grid; ~5.4 TB nodes still pass 2^53 in total
@@ -196,7 +263,20 @@ def regime(name: str):
     raise KeyError(name)
 
 
-REGIMES = ("a_totals", "a_totals_1800", "b_queues", "c_binpack", "c_spread", "c_edges", "c_edges_spread", "d_shares")
+REGIMES = ("a_totals", "a_totals_1800", "b_queues", "c_binpack", "c_spread", "c_edges", "c_edges_spread", "d_shares",
+           "e_overcommit", "e_overcommit_2048")
+
+
+def idle_gpu_key(snap: abi.Snapshot) -> np.ndarray:
+    """Idle + Releasing GPUs per node: the key of the idle-GPU scenario filter's top-k list."""
+    return snap.node_idle[abi.RES_GPU] + snap.node_releasing[abi.RES_GPU]
+
+
+def stripe_cut_goes_negative(snap: abi.Snapshot, nscan: int) -> bool:
+    """Some scanner of an `nscan`-scanner grid (one GPU: ranks j * nscan + my) holds >= 5 rows of which at most 3 have
+    a key >= 0: its 4th listed candidate is negative while it has more rows, so the list is cut at a negative key."""
+    key_by_rank = idle_gpu_key(snap)[np.argsort(snap.node_name_rank)]
+    return any(len(key_by_rank[my::nscan]) >= 5 and (key_by_rank[my::nscan] >= 0).sum() <= 3 for my in range(nscan))
 
 
 def without_pending(snap: abi.Snapshot) -> abi.Snapshot:
