@@ -390,9 +390,9 @@ __device__ Cand scan_tile_topk(const Tile &tl, const Decision &d, Cand *sh_warp,
   return best;  // valid on thread 0
 }
 
-// slot layout per CTA and parity (8 x u64):
-//   A {score bits, [tag:24][flags:8][repeat:8][rank:24]}
-//   B {cur_a gpu bits, tag}   C {cur_a cpu bits, tag}   D {repeat tracker-event bits, tag}
+// answer slot of a scanner in xbuf (8 x u64), read by the last CTA of the same launch after the ticket:
+//   single row {score bits, [flags:8][repeat:8][rank:24]} {cur_a gpu bits, cur_a cpu bits} {repeat tracker-event bits, -}
+//   min-max    {gpu min, count} {gpu max, count} {cpu min, count} {cpu max, count}
 constexpr int kSlotWords = 8;
 
 // candidate of this CTA -> slot words, including the same-node repeat analysis (lane 0 of warp 0)
@@ -400,7 +400,7 @@ constexpr int kSlotWords = 8;
 // (i = 0 is the swept placement, i >= 1 are candidate repeats on the same node); lane 0 then walks the
 // placements in order to simulate the min/max trackers and decides how many repeats it can vouch for.
 __device__ void publish_candidate(const Track *trk, const Tile &tl, const Decision &d, Cand local,
-                                  unsigned long long *slot, unsigned int tag, int batching, long long *dbg = nullptr) {
+                                  unsigned long long *slot, int batching, long long *dbg = nullptr) {
   const int lane = threadIdx.x & 31;
   long long d0 = clock64(), d1 = d0, d2 = d0, d3 = d0;
   local.score = __shfl_sync(0xffffffffu, local.score, 0);
@@ -556,12 +556,11 @@ __device__ void publish_candidate(const Track *trk, const Tile &tl, const Decisi
     dbg[1] += d2 - d1;
     dbg[2] += d3 - d2;
   }
-  st_relaxed_b128(slot + 2, (unsigned long long)__double_as_longlong(a_gpu), (unsigned long long)tag);
-  st_relaxed_b128(slot + 4, (unsigned long long)__double_as_longlong(a_cpu), (unsigned long long)tag);
-  if (repeat) st_relaxed_b128(slot + 6, rep_flags, (unsigned long long)tag);
-  unsigned long long hi = ((unsigned long long)tag << 40) | ((unsigned long long)(flags & 0xffu) << 32) |
-                          ((unsigned long long)(repeat & 0xffu) << 24) | (unsigned long long)(local.rank & 0xffffffu);
-  st_relaxed_b128(slot, (unsigned long long)__double_as_longlong(local.score), hi);
+  st_relaxed_b128(slot + 2, (unsigned long long)__double_as_longlong(a_gpu), (unsigned long long)__double_as_longlong(a_cpu));
+  if (repeat) st_relaxed_b128(slot + 4, rep_flags, 0ull);
+  unsigned long long meta = ((unsigned long long)(flags & 0xffu) << 32) | ((unsigned long long)(repeat & 0xffu) << 24) |
+                            (unsigned long long)(local.rank & 0xffffffu);
+  st_relaxed_b128(slot, (unsigned long long)__double_as_longlong(local.score), meta);
 }
 
 
@@ -573,7 +572,7 @@ __device__ void publish_candidate(const Track *trk, const Tile &tl, const Decisi
 // ---------------------------------------------------------------------------------------------
 enum { LF_TO_IDLE = 1, LF_EXHAUSTED = 2, LF_MORE = 4, LF_HAS_GPU = 8, LF_HAS_CPU = 16 };
 __device__ void publish_list_candidate(const Tile &tl, const Decision &d, Cand c, bool more, unsigned long long *line0_word,
-                                       unsigned long long *payload_line, unsigned int tag, double topo_term = 0.0) {
+                                       unsigned long long *payload_line, double topo_term = 0.0) {
   const int lane = threadIdx.x & 31;
   uint32_t flags = more ? LF_MORE : 0u, repeat = 0;
   double Ig0 = 0, Lg0 = 0, Ic0 = 0, Lc0 = 0;
@@ -657,25 +656,23 @@ __device__ void publish_list_candidate(const Tile &tl, const Decision &d, Cand c
     if (!((fit_mask >> (r_n + 1)) & 1u)) flags |= LF_EXHAUSTED;  // after 1 + repeat placements the row no longer fits
   }
   if (lane == 0) {
-    st_relaxed_sys_b128(payload_line + 0, (unsigned long long)__double_as_longlong(Ig0), (unsigned long long)tag);
-    st_relaxed_sys_b128(payload_line + 2, (unsigned long long)__double_as_longlong(Lg0), (unsigned long long)tag);
-    st_relaxed_sys_b128(payload_line + 4, (unsigned long long)__double_as_longlong(Ic0), (unsigned long long)tag);
-    st_relaxed_sys_b128(payload_line + 6, (unsigned long long)__double_as_longlong(Lc0), (unsigned long long)tag);
-    unsigned long long hi = ((unsigned long long)tag << 40) | ((unsigned long long)(flags & 0xffu) << 32) |
-                            ((unsigned long long)(repeat & 0xffu) << 24) | (unsigned long long)(c.rank & 0xffffffu);
+    st_relaxed_sys_b128(payload_line + 0, (unsigned long long)__double_as_longlong(Ig0), (unsigned long long)__double_as_longlong(Lg0));
+    st_relaxed_sys_b128(payload_line + 2, (unsigned long long)__double_as_longlong(Ic0), (unsigned long long)__double_as_longlong(Lc0));
+    unsigned long long hi = ((unsigned long long)(flags & 0xffu) << 32) | ((unsigned long long)(repeat & 0xffu) << 24) |
+                            (unsigned long long)(c.rank & 0xffffffu);
     st_relaxed_sys_b128(line0_word, (unsigned long long)__double_as_longlong(c.score), hi);
   }
 }
 
 // =============================================================================================
-// device-side exchanges inside one launch
+// device-side exchange inside one launch
 // =============================================================================================
-// Watchdog for the spin waits: a wait that does not complete within ~2^22 polls records (code, seq, who)
+// Watchdog for the spin wait of the XB_FUSED_MM exchange: a wait that does not complete within ~2^22 polls records (code, seq, who)
 // in counters[24..27], raises the abort flag and lets every waiter fall through so that the kernel ends
 // and the host reports KAI_ERR_CUDA instead of hanging the GPU.
 struct Spin {
   unsigned int n = 0;
-  __device__ __forceinline__ bool expired(const ActionParams &p, int code, unsigned int seq, int who) {
+  __device__ __forceinline__ bool expired(const ActionParams &p, int code, unsigned long long seq, int who) {
     if ((++n & 0x3ffu) != 0) return false;
     volatile long long *c = p.counters;
     if (c[24] != 0) return true;
@@ -789,7 +786,7 @@ __device__ bool scanner_main(const ActionParams &p, const LaunchRec *lrec, unsig
     if (tid == 0) *(int *)gstate = -1;
     return false;
   }
-  const unsigned int seq = lrec->seq;
+  const unsigned long long seq = lrec->seq;
   long long ts[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   long long c0 = clock64();
   if (tid < kDecWords) sh.dw[tid] = lrec->dw[tid];
@@ -839,13 +836,12 @@ __device__ bool scanner_main(const ActionParams &p, const LaunchRec *lrec, unsig
       bool mine = false, ext = false;
       if (e < nd) {
         const unsigned long long lo = (unsigned long long)lrec->dkey[e] | ((unsigned long long)lrec->dtask[e] << 32);
-        const unsigned long long hi = (unsigned long long)seq | ((unsigned long long)lrec->dcount[e] << 32);
         int2 en = make_int2((int)(unsigned int)(lo & 0xffffffffu), (int)(unsigned int)(lo >> 32));
         sh.delta[e] = en;
         int ln = 0;
         ext = en.x < 0;
         mine = en.x >= 0 && tile_owns(tile, (unsigned int)(en.x & 0x0fffffff), ln) && ln < tile.count;
-        sh.dln[e] = ln | ((int)(hi >> 32) << 24);  // repeat count - 1 in the top byte
+        sh.dln[e] = ln | ((int)lrec->dcount[e] << 24);  // repeat count - 1 in the top byte
         if (mine && ((en.x >> 28) & 7) < ND_FEAS_SET)
           for (int r = 0; r < s.R; r++) sh.dreq[e][r] = __ldg(&s.t_req[(size_t)en.y * s.R + r]);
       }
@@ -939,7 +935,7 @@ __device__ bool scanner_main(const ActionParams &p, const LaunchRec *lrec, unsig
       if (tid == 0) tile_carve(tile, smem);
       __syncthreads();
     }
-    unsigned long long *slot = p.xbuf + (size_t)(seq & 1) * kMaxGrid * kSlotWords + (size_t)my * kSlotWords;
+    unsigned long long *slot = p.xbuf + (size_t)my * kSlotWords;
     if (!p.fused_in_kernel && kind == DK_SCAN && (sh.xbits & XB_FUSED_MM)) {
       // the extremes of this row set were reduced by the MINMAX launch that precedes this one on the stream
       if (tid == 0) {
@@ -975,12 +971,14 @@ __device__ bool scanner_main(const ActionParams &p, const LaunchRec *lrec, unsig
           sh_d[warp * 4 + 3] = mx[1];
         }
         __syncthreads();
-        unsigned long long *mmbase = p.mmbuf + (size_t)(seq & 1) * kMaxGrid * kSlotWords;
+        // the one wait inside a launch: every scanner's extremes, tagged with the full sequence number (a slot of an
+        // earlier record never matches), under the watchdog so that a protocol bug ends the kernel
+        unsigned long long *mmbase = p.mmbuf;
         if (tid < 4) {
           double v = tid & 1 ? 0.0 : DBL_MAX;
           for (int w = 0; w < nw; w++) v = tid & 1 ? fmax(v, sh_d[w * 4 + tid]) : fmin(v, sh_d[w * 4 + tid]);
           st_relaxed_b128(mmbase + (size_t)my * kSlotWords + 2 * tid, (unsigned long long)__double_as_longlong(v),
-                          (unsigned long long)seq);
+                          seq);
         }
         __syncthreads();
         double g[4] = {DBL_MAX, 0.0, DBL_MAX, 0.0};
@@ -990,7 +988,7 @@ __device__ bool scanner_main(const ActionParams &p, const LaunchRec *lrec, unsig
             Spin spin;
             do {
               ld_relaxed_b128(mmbase + (size_t)c * kSlotWords + 2 * i, lo, hi);
-            } while (hi != (unsigned long long)seq && !spin.expired(p, 14, seq, c));
+            } while (hi != seq && !spin.expired(p, 14, seq, c));
             double v = __longlong_as_double((long long)lo);
             g[i] = i & 1 ? fmax(g[i], v) : fmin(g[i], v);
           }
@@ -1026,7 +1024,7 @@ __device__ bool scanner_main(const ActionParams &p, const LaunchRec *lrec, unsig
         __syncthreads();
       }
       if (tid == 0) ts[4] += clock64() - c3;
-      unsigned long long *lines = p.d_list + ((size_t)(seq & 1) * kListScanners + (size_t)my) * kListLines * kListLineWords;
+      unsigned long long *lines = p.d_list + (size_t)my * kListLines * kListLineWords;
       if (warp < kTopM) {
         double topo_term = 0.0;
         if (sh.pref_level >= 0 && sh.cands[warp].rank != kRankNone) {
@@ -1034,7 +1032,7 @@ __device__ bool scanner_main(const ActionParams &p, const LaunchRec *lrec, unsig
           topo_term = __dmul_rn((double)((dd >= 0 && dd < kDomBuckets) ? sh.dom_bucket[dd] : 0), 10000.0);
         }
         publish_list_candidate(tile, sh.dec, sh.cands[warp], sh.fit_count > kTopM, lines + 2 * warp,
-                               lines + (size_t)(1 + warp) * kListLineWords, seq & 0xffffffu, topo_term);
+                               lines + (size_t)(1 + warp) * kListLineWords, topo_term);
       }
     } else if (kind == DK_TOPK) {
       // ---- accumulated_scenario_filters/idle_gpus: rows by idle + releasing GPUs, descending (name rank ascending
@@ -1049,19 +1047,18 @@ __device__ bool scanner_main(const ActionParams &p, const LaunchRec *lrec, unsig
         }
         __syncthreads();
       }
-      unsigned long long *lines = p.d_list + ((size_t)(seq & 1) * kListScanners + (size_t)my) * kListLines * kListLineWords;
+      unsigned long long *lines = p.d_list + (size_t)my * kListLines * kListLineWords;
       if (tid < kTopM) {
         const Cand c = sh.cands[tid];
         const uint32_t flags = sh.fit_count > kTopM ? LF_MORE : 0u;
-        unsigned long long hi = ((unsigned long long)(seq & 0xffffffu) << 40) | ((unsigned long long)flags << 32) |
-                                (unsigned long long)(c.rank == kRankNone ? kRankNone : (c.rank & 0xffffffu));
+        unsigned long long hi = ((unsigned long long)flags << 32) | (unsigned long long)(c.rank == kRankNone ? kRankNone : (c.rank & 0xffffffu));
         st_relaxed_sys_b128(lines + 2 * tid, (unsigned long long)__double_as_longlong(c.score), hi);
       }
     } else if (kind == DK_SCAN) {
       Cand local = scan_tile(tile, sh.dec, s, sh_warp, nullptr, 0, nullptr, sh.xbits, sh.pref_level, sh.dom_bucket);
       long long c4 = clock64();
       if (tid == 0) ts[4] += c4 - c3;
-      if (warp == 0) publish_candidate(sh.trk, tile, sh.dec, local, slot, seq & 0xffffffu, sh.batching, my == 0 ? p.counters + 40 : nullptr);
+      if (warp == 0) publish_candidate(sh.trk, tile, sh.dec, local, slot, sh.batching, my == 0 ? p.counters + 40 : nullptr);
     } else if (kind == DK_MINMAX) {
       double mn[2] = {DBL_MAX, DBL_MAX}, mx[2] = {0, 0};
       for (int ln = tid; ln < tile.count; ln += blockDim.x)
@@ -1114,20 +1111,10 @@ __device__ bool scanner_main(const ActionParams &p, const LaunchRec *lrec, unsig
         int tot[4] = {0, 0, 0, 0};
         for (int w = 0; w < nw; w++)
           for (int i = 0; i < 4; i++) tot[i] += sh_i[w * 4 + i];
-        unsigned long long tag = seq;
-        slot = p.mmbuf + (size_t)(seq & 1) * kMaxGrid * kSlotWords + (size_t)my * kSlotWords;
-        auto put = [&](unsigned long long *w, unsigned long long lo, unsigned long long hi2) {
-          st_relaxed_b128(w, lo, hi2);
-        };
-        put(slot + 0, (unsigned long long)__double_as_longlong(mn[0]), (tag << 32) | (unsigned int)tot[0]);
-        put(slot + 2, (unsigned long long)__double_as_longlong(mx[0]), (tag << 32) | (unsigned int)tot[1]);
-        put(slot + 4, (unsigned long long)__double_as_longlong(mn[1]), (tag << 32) | (unsigned int)tot[2]);
-        put(slot + 6, (unsigned long long)__double_as_longlong(mx[1]), (tag << 32) | (unsigned int)tot[3]);
-      }
-    } else {  // DK_FLUSH: acknowledge
-      if (tid == 0) {
-        unsigned long long hi = ((unsigned long long)(seq & 0xffffffu) << 40) | (unsigned long long)kRankNone;
-        st_relaxed_b128(slot, (unsigned long long)__double_as_longlong(-1.0), hi);
+        st_relaxed_b128(slot + 0, (unsigned long long)__double_as_longlong(mn[0]), (unsigned long long)(unsigned int)tot[0]);
+        st_relaxed_b128(slot + 2, (unsigned long long)__double_as_longlong(mx[0]), (unsigned long long)(unsigned int)tot[1]);
+        st_relaxed_b128(slot + 4, (unsigned long long)__double_as_longlong(mn[1]), (unsigned long long)(unsigned int)tot[2]);
+        st_relaxed_b128(slot + 6, (unsigned long long)__double_as_longlong(mx[1]), (unsigned long long)(unsigned int)tot[3]);
       }
     }
     if (tid == 0) {
@@ -1162,73 +1149,61 @@ __device__ bool scanner_main(const ActionParams &p, const LaunchRec *lrec, unsig
 // the last CTA of a launch
 // =============================================================================================
 // Reduce the scanners' answers for record `seq` on the GPU and write ONE 64-byte line to host memory (a host
-// core pays ~80 ns per GPU-written cache line it reads; 147 lines per sweep were the bottleneck).
-__device__ void reduce_answers(const ActionParams &p, int kind, unsigned int seq) {
+// core pays ~80 ns per GPU-written cache line it reads; 147 lines per sweep were the bottleneck).  The scanners wrote
+// their slots before taking the ticket, so they are read once.  The line is the payload, then, after a system fence,
+// the sequence number in its last word.
+__device__ void reduce_answers(const ActionParams &p, int kind, unsigned long long seq) {
   const int lane = threadIdx.x & 31;
   const int n = p.scanners;
-  if (kind == DK_SCAN || kind == DK_FLUSH) {
-    const unsigned long long *buf = p.xbuf + (size_t)(seq & 1) * kMaxGrid * kSlotWords;
-    const unsigned int tag = seq & 0xffffffu;
+  const unsigned long long *buf = p.xbuf;
+  unsigned long long *out = (kind == DK_SCAN ? p.h_slot : p.h_mmslot) + (size_t)(seq & 1) * p.cfg.shard_count * kLineWords;
+  if (kind == DK_SCAN) {
     double bs = -1.0;
     uint32_t brank = kRankNone;
-    unsigned long long bhi = ((unsigned long long)tag << 40) | (unsigned long long)kRankNone;
+    unsigned long long bmeta = (unsigned long long)kRankNone;
     int bslot = -1;
     for (int c = lane; c < n; c += 32) {
       unsigned long long lo, hi;
-      Spin spin;
-      do {
-        ld_relaxed_b128(buf + (size_t)c * kSlotWords, lo, hi);
-      } while ((unsigned int)(hi >> 40) != tag && !spin.expired(p, 13, seq, c));
+      ld_relaxed_b128(buf + (size_t)c * kSlotWords, lo, hi);
       double sc = __longlong_as_double((long long)lo);
       uint32_t rk = (uint32_t)(hi & 0xffffffu);
       if (better(sc, rk, bs, brank)) {
         bs = sc;
         brank = rk;
-        bhi = hi;
+        bmeta = hi;
         bslot = c;
       }
     }
     for (int o = 16; o > 0; o >>= 1) {
       double os = __shfl_xor_sync(0xffffffffu, bs, o);
       uint32_t orank = __shfl_xor_sync(0xffffffffu, brank, o);
-      unsigned long long ohi = __shfl_xor_sync(0xffffffffu, bhi, o);
+      unsigned long long ometa = __shfl_xor_sync(0xffffffffu, bmeta, o);
       int osl = __shfl_xor_sync(0xffffffffu, bslot, o);
       if (better(os, orank, bs, brank)) {
         bs = os;
         brank = orank;
-        bhi = ohi;
+        bmeta = ometa;
         bslot = osl;
       }
     }
-    unsigned long long *out = p.h_slot + (size_t)(seq & 1) * kMaxGrid * kSlotWords;
-    if (brank != kRankNone && lane >= 1 && lane <= 3) {  // payload words B, C, D of the winning slot
-      const uint32_t repeat = (uint32_t)((bhi >> 24) & 0xffu);
-      if (lane < 3 || repeat) {
-        unsigned long long lo, hi;
-        Spin spin;
-        do {
-          ld_relaxed_b128(buf + (size_t)bslot * kSlotWords + 2 * lane, lo, hi);
-        } while ((unsigned int)hi != tag && !spin.expired(p, 14, seq, bslot));
-        st_relaxed_sys_b128(out + 2 * lane, lo, hi);
+    if (lane == 0) {  // the winning slot's cur_a values and repeat events
+      unsigned long long ag = 0, ac = 0, rep = 0, unused;
+      if (brank != kRankNone) {
+        ld_relaxed_b128(buf + (size_t)bslot * kSlotWords + 2, ag, ac);
+        if ((bmeta >> 24) & 0xffu) ld_relaxed_b128(buf + (size_t)bslot * kSlotWords + 4, rep, unused);
       }
+      st_relaxed_sys_b128(out, (unsigned long long)__double_as_longlong(bs), bmeta);
+      st_relaxed_sys_b128(out + 2, ag, ac);
+      st_relaxed_sys_b128(out + 4, rep, 0ull);
     }
-    __syncwarp();
-    if (lane == 0) st_relaxed_sys_b128(out, (unsigned long long)__double_as_longlong(bs), bhi);
   } else if (kind == DK_MINMAX) {
-    const unsigned long long *buf = p.mmbuf + (size_t)(seq & 1) * kMaxGrid * kSlotWords;
-    const unsigned long long tag = seq;
     double gmn[2] = {DBL_MAX, DBL_MAX}, gmx[2] = {0, 0};
     long long cmn[2] = {0, 0}, cmx[2] = {0, 0};
     for (int cta = lane; cta < n; cta += 32) {
       const unsigned long long *slot = buf + (size_t)cta * kSlotWords;
       for (int k = 0; k < 2; k++) {
         unsigned long long lo, hi;
-        {
-          Spin spin;
-          do {
-            ld_relaxed_b128(slot + 4 * k, lo, hi);
-          } while ((hi >> 32) != (tag & 0xffffffffu) && !spin.expired(p, 15, seq, cta));
-        }
+        ld_relaxed_b128(slot + 4 * k, lo, hi);
         double v = __longlong_as_double((long long)lo);
         int cnt = (int)(hi & 0xffffffffu);
         if (cnt > 0) {
@@ -1238,12 +1213,7 @@ __device__ void reduce_answers(const ActionParams &p, int kind, unsigned int seq
           } else if (v == gmn[k])
             cmn[k] += cnt;
         }
-        {
-          Spin spin;
-          do {
-            ld_relaxed_b128(slot + 4 * k + 2, lo, hi);
-          } while ((hi >> 32) != (tag & 0xffffffffu) && !spin.expired(p, 16, seq, cta));
-        }
+        ld_relaxed_b128(slot + 4 * k + 2, lo, hi);
         v = __longlong_as_double((long long)lo);
         cnt = (int)(hi & 0xffffffffu);
         if (cnt > 0) {
@@ -1276,21 +1246,24 @@ __device__ void reduce_answers(const ActionParams &p, int kind, unsigned int seq
             cmx[k] += ocmx;
         }
       }
-    if (lane == 0) {  // the next launch (XB_FUSED_MM sweep) reads the extremes on the device
-      for (int k = 0; k < 2; k++) {
-        p.mm_result[2 * k] = cmn[k] > 0 ? gmn[k] : DBL_MAX;
-        p.mm_result[2 * k + 1] = cmx[k] > 0 ? gmx[k] : 0.0;
-      }
-    }
     if (lane == 0) {
-      unsigned long long *out = p.h_mmslot + (size_t)(seq & 1) * kMaxGrid * kSlotWords;
+      unsigned long long cnt[2];
       for (int k = 0; k < 2; k++) {
-        unsigned int c0 = (unsigned int)(cmn[k] > 0x7fffffff ? 0x7fffffff : cmn[k]);
-        unsigned int c1 = (unsigned int)(cmx[k] > 0x7fffffff ? 0x7fffffff : cmx[k]);
-        st_relaxed_sys_b128(out + 4 * k, (unsigned long long)__double_as_longlong(gmn[k]), (tag << 32) | c0);
-        st_relaxed_sys_b128(out + 4 * k + 2, (unsigned long long)__double_as_longlong(gmx[k]), (tag << 32) | c1);
+        p.mm_result[2 * k] = cmn[k] > 0 ? gmn[k] : DBL_MAX;  // the next launch (XB_FUSED_MM sweep) reads the extremes
+        p.mm_result[2 * k + 1] = cmx[k] > 0 ? gmx[k] : 0.0;
+        const unsigned int c0 = (unsigned int)(cmn[k] > 0x7fffffff ? 0x7fffffff : cmn[k]);
+        const unsigned int c1 = (unsigned int)(cmx[k] > 0x7fffffff ? 0x7fffffff : cmx[k]);
+        cnt[k] = (unsigned long long)c0 | ((unsigned long long)c1 << 32);
       }
+      // {gpu min, gpu max} {cpu min, cpu max} {gpu counts at min | at max << 32, cpu counts}
+      st_relaxed_sys_b128(out, (unsigned long long)__double_as_longlong(gmn[0]), (unsigned long long)__double_as_longlong(gmx[0]));
+      st_relaxed_sys_b128(out + 2, (unsigned long long)__double_as_longlong(gmn[1]), (unsigned long long)__double_as_longlong(gmx[1]));
+      st_relaxed_sys_b128(out + 4, cnt[0], cnt[1]);
     }
+  }
+  if (lane == 0) {
+    __threadfence_system();  // the payload is out before the sequence number
+    st_relaxed_sys_b128(out + kLineWords - 2, 0ull, seq);
   }
   __syncwarp();
 }
@@ -1319,7 +1292,7 @@ __device__ __forceinline__ bool mk_before(unsigned long long ah, unsigned long l
 constexpr int kMergeCtas = 4, kMergeCtaThreads = kMergeThreads / kMergeCtas;
 constexpr size_t kMergeCtaSmemBytes = (size_t)kMergeCtaThreads * 8 * (2 + kCEntryWords);
 __global__ void __cluster_dims__(kMergeCtas, 1, 1) __launch_bounds__(kMergeCtaThreads, 1)
-    k_merge_cluster(const __grid_constant__ ActionParams p, unsigned int seq, int with_payload) {
+    k_merge_cluster(const __grid_constant__ ActionParams p, unsigned long long seq, int with_payload) {
   namespace cg = cooperative_groups;
   cg::cluster_group cluster = cg::this_cluster();
   extern __shared__ __align__(16) unsigned char dyn_smem[];
@@ -1335,7 +1308,7 @@ __global__ void __cluster_dims__(kMergeCtas, 1, 1) __launch_bounds__(kMergeCtaTh
   const int g = (int)crank * kMergeCtaThreads + tid;  // my position in the network
   const int n_scan = p.scanners;
   const int n_c = n_scan * kTopM;
-  const unsigned long long *base = p.d_list + (size_t)(seq & 1) * kListScanners * kListLines * kListLineWords;
+  const unsigned long long *base = p.d_list;
   const long long t0 = clock64();
   unsigned long long h = ~0ull, l = ~0ull;
   bool more = false;
@@ -1452,19 +1425,18 @@ __global__ void __cluster_dims__(kMergeCtas, 1, 1) __launch_bounds__(kMergeCtaTh
     const int c = src / kTopM, m = src % kTopM;
     const unsigned long long *lines = base + (size_t)c * kListLines * kListLineWords;
     const uint4 v = __ldcg((const uint4 *)(lines + 2 * m));
-    uint4 pw[4];
-#pragma unroll
-    for (int q = 0; q < 4; q++) pw[q] = make_uint4(0, 0, 0, 0);
-    if (with_payload) {
-      const unsigned long long *pl = lines + (size_t)(1 + m) * kListLineWords;
-#pragma unroll
-      for (int q = 0; q < 4; q++) pw[q] = __ldcg((const uint4 *)(pl + 2 * q));
-    }
     unsigned long long *e = stage + (size_t)tid * kCEntryWords;
     e[0] = (unsigned long long)v.x | ((unsigned long long)v.y << 32);
     e[1] = (unsigned long long)v.z | ((unsigned long long)v.w << 32);
-#pragma unroll
-    for (int q = 0; q < 4; q++) e[2 + q] = (unsigned long long)pw[q].x | ((unsigned long long)pw[q].y << 32);
+    for (int q = 2; q < kCEntryWords; q++) e[q] = 0;
+    if (with_payload) {  // {Ig, Lg} {Ic, Lc}
+      const ulonglong2 *pl = (const ulonglong2 *)(lines + (size_t)(1 + m) * kListLineWords);
+      const ulonglong2 g = __ldcg(pl), c2 = __ldcg(pl + 1);
+      e[2] = g.x;
+      e[3] = g.y;
+      e[4] = c2.x;
+      e[5] = c2.y;
+    }
   }
   __syncthreads();
   const int first = (int)crank * kMergeCtaThreads;
@@ -1476,7 +1448,7 @@ __global__ void __cluster_dims__(kMergeCtas, 1, 1) __launch_bounds__(kMergeCtaTh
   cluster.sync();
   if (crank == 0 && tid == 0) {
     __threadfence_system();
-    st_relaxed_sys_b128(out, (unsigned long long)(unsigned int)n_out | (have_cut ? (1ull << 31) : 0ull), (unsigned long long)seq);
+    st_relaxed_sys_b128(out, (unsigned long long)(unsigned int)n_out | (have_cut ? (1ull << 31) : 0ull), seq);
     const long long t3 = clock64();
     p.counters[44] += t3 - t0;
     p.counters[45] += 1;

@@ -24,8 +24,8 @@ constexpr uint32_t kNoRank = 0xFFFFFFFFu;
 constexpr int kDecWords = 16;         // tagged words of one decision record
 constexpr int kMaxDelta = 256;        // node deltas carried by one decision record
 constexpr int kTopM = 4;              // candidates every scanner returns per list sweep
-constexpr int kListScanners = 2048;   // scanner lines per parity of d_list
-constexpr int kListLineWords = 8;     // one 64-byte line = 4 tagged words
+constexpr int kListScanners = 2048;   // scanner lines of d_list
+constexpr int kListLineWords = 8;     // one 64-byte line
 constexpr int kListLines = 1 + kTopM; // line 0: the M candidate words, lines 1..M: row values of candidate m
 constexpr int kMaxDomLevels = 8;      // topology levels of all Topology CRs together (rows keep one domain id per level)
 constexpr int kDomBuckets = 4096;     // preferred-level domains that can carry a node score at a time
@@ -300,13 +300,15 @@ struct ActionParams {
   kai_config cfg;
   int scanners;              // CTAs of k_record
   int nodes_per_cta;         // node rows per scanner (tile height)
-  unsigned long long *xbuf;  // exchange slots: [2][kMaxGrid][8] u64 (tagged 128-bit words A, B, C, D)
-  unsigned long long *mmbuf; // min/max exchange: [2][kMaxGrid][8] u64
+  unsigned long long *xbuf;  // answer slots of the scanners (single row / min-max): [kMaxGrid][8] u64
+  unsigned long long *mmbuf; // XB_FUSED_MM exchange inside one launch: [kMaxGrid][8] u64, tagged with the sequence number
   long long *counters;       // [48]: watchdog (24..27) and KAI_PROFILE cycle counts
-  unsigned long long *h_slot, *h_mmslot;  // this GPU's reduced answer line [2][kSlotWords] in (shared) host memory
+  // this GPU's reduced single-row / min-max answer line in (shared) host memory: lines [2][ranks][kLineWords], parity by
+  // sequence number, this GPU's line of parity 0
+  unsigned long long *h_slot, *h_mmslot;
   int spin_log2;             // watchdog: polls before a wait is declared dead
   int topm;                  // scanners answer with their kTopM best rows (0 = single best through the last CTA)
-  unsigned long long *d_list;  // [2][kListScanners][kListLines][kListLineWords]: the scanners' top-M lines
+  unsigned long long *d_list;  // [kListScanners][kListLines][kListLineWords]: the scanners' top-M lines
   const int *node_domain;    // [n_dom_levels][N] topology domain of every node per level (-1 = label missing), or null
   int n_dom_levels;
   unsigned char *g_tiles;      // [scanners][g_tile_stride] tiles in the layout of tile_carve
@@ -320,7 +322,10 @@ struct ActionParams {
 
 constexpr int kMergeCap = 1024;                      // candidates k_merge_cluster sorts, one per thread (scanners x kTopM)
 constexpr int kCEntryWords = 6;                      // score, meta, Ig, Lg, Ic, Lc
-constexpr int kCListWords = 2 + kMergeCap * kCEntryWords;  // header {count | more << 31, tag} + entries
+constexpr int kCListWords = 2 + kMergeCap * kCEntryWords;  // header {count | more << 31, sequence number} + entries
+// A single-row or min-max answer line in host memory: payload words, then the record's sequence number in the last word,
+// written after a system fence (the host waits on that word alone)
+constexpr int kLineWords = 8;
 constexpr int kScanStateBytes = 16 + kDomBuckets;
 constexpr int kMaxDeltaL = kMaxDelta;
 enum { DK_LOAD = 6 };  // load the tiles from the session tables (first launch of an action)
@@ -328,7 +333,7 @@ enum { DK_LOAD = 6 };  // load the tiles from the session tables (first launch o
 // One decision record, passed to k_record by value in the kernel parameter space.
 struct LaunchRec {
   unsigned long long dw[kDecWords];
-  unsigned int seq;
+  uint64_t seq;
   int n_delta;
   unsigned int dkey[kMaxDeltaL];    // name rank | code << 28, or an extended entry (bit 31)
   unsigned int dtask[kMaxDeltaL];

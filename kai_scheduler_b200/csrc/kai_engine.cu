@@ -90,8 +90,9 @@ struct Staging {  // pinned host staging buffer mirrored 1:1 onto a device arena
 size_t align_up(size_t v, size_t a) { return (v + a - 1) & ~(a - 1); }
 
 constexpr int kShmRanks = 16;  // GPUs of one box that can share the exchange segment
-// layout of the shared exchange segment (u64 words): answer lines | min/max lines | merged lists per rank
-size_t shm_clist_offset_words() { return (size_t)2 * 2 * kMaxGrid * kSlotWords; }
+// layout of the shared exchange segment (u64 words): answer lines | min/max lines, each [2][ranks][kLineWords] in room
+// for kShmRanks ranks | merged lists per rank
+size_t shm_clist_offset_words() { return (size_t)2 * 2 * kShmRanks * kLineWords; }
 
 }  // namespace
 
@@ -131,7 +132,7 @@ struct kai_engine {
   long long record_launches = 0;
   // multi-GPU (one engine per process per GPU): the reduced answer lines of all GPUs live in one POSIX shm
   // segment that every process maps and registers with CUDA; each host sequencer reads all lines.
-  unsigned long long *shm_base = nullptr;  // [slots | mm], each [2][kMaxGrid][kSlotWords]
+  unsigned long long *shm_base = nullptr;  // [slots | mm | lists], see shm_clist_offset_words()
   size_t shm_bytes = 0;
   char shm_name[48] = {0};
   bool shm_owner = false, shm_registered = false;
@@ -165,7 +166,7 @@ struct kai_engine {
   long long *counters = nullptr;
   kai_job_visit *d_visits = nullptr;
   double *fs_w = nullptr, *fs_rr = nullptr;
-  unsigned int seq = 2;
+  uint64_t seq = 2;  // sequence number of the next answered record: grows across actions and loads, never restarts
 
   // host result buffers (pinned)
   Staging rstage;
@@ -264,37 +265,11 @@ static void structure_checksums(const kai_snapshot *s, std::vector<uint64_t> &ou
   for_each_structural_field(s, [&](const char *, const void *p, size_t bytes) { out.push_back(checksum_bytes(p, bytes)); });
 }
 
-// Host sequencer / scanner protocol: decision records, answer slots and candidate lines carry the sequence number of
-// the record they belong to (24-bit tags in the slots and lines, the full 32 bits in the merged lists), and the number
-// keeps growing across actions and loads so that a line left over from an earlier record can never match.  Past the
-// threshold (1 << 22, KAI_SEQ_RESET_AT overrides it for tests) every tagged buffer is cleared and numbering restarts,
-// long before a 24-bit tag could repeat.  Several GPUs (shard_count > 1) share the exchange segment and would have to
-// agree on the restart; they never reset, so after 2^24 records a line left untouched since exactly 2^24 records ago
-// could be taken as current.
-static int reset_sequence_if_due(kai_engine *e) {
-  unsigned long long at = 1ull << 22;
-  if (const char *v = getenv("KAI_SEQ_RESET_AT")) {
-    long long x = atoll(v);
-    if (x >= 2) at = (unsigned long long)x;
-  }
-  if (e->seq <= at || e->cfg.shard_count != 1) return KAI_OK;
-  e->seq = 2;
-  memset(e->h_pinned, 0, ((size_t)2 * kMaxDelta * 2 + (size_t)2 * 2 * kMaxGrid * kSlotWords) * 8);
-  memset(e->h_clist, 0, (size_t)2 * kCListWords * 8);
-  const size_t list_words = (size_t)2 * kListScanners * kListLines * kListLineWords, xb = (size_t)2 * kMaxGrid * 8 * 8;
-  if (e->d_list) CK(cudaMemsetAsync(e->d_list, 0, list_words * 8, e->stream));
-  if (e->mm_result) CK(cudaMemsetAsync(e->mm_result, 0, 32, e->stream));
-  if (e->xbuf) CK(cudaMemsetAsync(e->xbuf, 0, xb, e->stream));
-  if (e->mmbuf) CK(cudaMemsetAsync(e->mmbuf, 0, xb, e->stream));
-  return KAI_OK;
-}
-
 static int load_tail(kai_engine *e, const kai_snapshot *s, int n_dom_levels, bool resident) {
   const int N = e->N, T = e->T, Q = e->Q;
   const DevSnap &ds = e->ds;
   const size_t RN = (size_t)e->R * N, QN = (size_t)QR * Q;
   (void)RN;
-  if (int rc = reset_sequence_if_due(e)) return rc;
   // ---------------- open session: totals, queue usage, fair share ----------------
   if (N > 0) {
     int blocks = std::min(e->num_sms * 4, (N + 255) / 256);
@@ -402,7 +377,7 @@ int kai_engine_create(const kai_config *cfg, kai_engine **out) {
   for (auto &ev : e->ev) cudaEventCreate(&ev);
   cudaEventCreateWithFlags(&e->ev_mirror, cudaEventDisableTiming);
   {  // pinned, device-mapped buffers of the host sequencer
-    size_t words = (size_t)2 * kMaxDelta * 2 + (size_t)2 * 2 * kMaxGrid * kSlotWords;
+    size_t words = (size_t)2 * kMaxDelta * 2 + (size_t)2 * 2 * kLineWords;
     if (cudaHostAlloc((void **)&e->h_pinned, words * 8, cudaHostAllocMapped | cudaHostAllocPortable) != cudaSuccess) {
       delete e;
       return KAI_ERR_CUDA;
@@ -410,7 +385,7 @@ int kai_engine_create(const kai_config *cfg, kai_engine **out) {
     memset(e->h_pinned, 0, words * 8);
     e->h_delta = e->h_pinned;
     e->h_slots = e->h_delta + (size_t)2 * kMaxDelta * 2;
-    e->h_mm = e->h_slots + (size_t)2 * kMaxGrid * kSlotWords;
+    e->h_mm = e->h_slots + (size_t)2 * kLineWords;
     if (cudaHostAlloc((void **)&e->h_clist, (size_t)2 * kCListWords * 8, cudaHostAllocMapped | cudaHostAllocPortable) != cudaSuccess) {
       delete e;
       return KAI_ERR_CUDA;
@@ -948,7 +923,7 @@ int kai_engine_load_snapshot(kai_engine *e, const kai_snapshot *s) {
     e->lnpc = lnpc;
     e->ltile_bytes = ltile_bytes;
     e->ltile_stride = align_up(ltile_bytes, 256);
-    const size_t list_words = (size_t)2 * kListScanners * kListLines * kListLineWords;
+    const size_t list_words = (size_t)kListScanners * kListLines * kListLineWords;
     CK(e->dlaunch.reserve((size_t)lg * e->ltile_stride + (size_t)lg * align_up(kScanStateBytes, 256) + list_words * 8 + 4096));
     e->g_tiles = e->dlaunch.take<unsigned char>((size_t)lg * e->ltile_stride);
     e->g_scan_state = e->dlaunch.take<unsigned char>((size_t)lg * kScanStateBytes);
@@ -960,11 +935,11 @@ int kai_engine_load_snapshot(kai_engine *e, const kai_snapshot *s) {
     CK(cudaMemsetAsync(e->mm_result, 0, 32, e->stream));
   }
   {
-    size_t xb = (size_t)2 * kMaxGrid * 8 * 8;
+    size_t xb = (size_t)kMaxGrid * kSlotWords * 8;
     size_t misc = 2 * xb + 256 + sizeof(long long) * 48 + sizeof(kai_job_visit) * (size_t)e->visits_cap + 2 * QN * 8 + 4096;
     CK(e->dmisc.reserve(misc));
-    e->xbuf = e->dmisc.take<unsigned long long>(2 * kMaxGrid * 8);
-    e->mmbuf = e->dmisc.take<unsigned long long>(2 * kMaxGrid * 8);
+    e->xbuf = e->dmisc.take<unsigned long long>((size_t)kMaxGrid * kSlotWords);
+    e->mmbuf = e->dmisc.take<unsigned long long>((size_t)kMaxGrid * kSlotWords);
     e->counters = e->dmisc.take<long long>(48);
     e->d_visits = e->dmisc.take<kai_job_visit>(e->visits_cap);
     e->fs_w = e->dmisc.take<double>(QN + 1);
@@ -1097,9 +1072,9 @@ int kai_engine_run(kai_engine *e, kai_action action, kai_result *out) {
   const int batching = getenv("KAI_NO_BATCHING") ? 0 : 1;
   // one reduced answer line and one merged list per GPU; with several GPUs they live in the shared segment
   unsigned long long *lines = e->cfg.shard_count > 1 ? e->shm_dev : e->h_slots;
-  unsigned long long *mm_lines = e->cfg.shard_count > 1 ? e->shm_dev + (size_t)2 * kMaxGrid * kSlotWords : e->h_mm;
-  p.h_slot = lines + (size_t)e->cfg.shard_rank * kSlotWords;
-  p.h_mmslot = mm_lines + (size_t)e->cfg.shard_rank * kSlotWords;
+  unsigned long long *mm_lines = e->cfg.shard_count > 1 ? e->shm_dev + (size_t)2 * kShmRanks * kLineWords : e->h_mm;
+  p.h_slot = lines + (size_t)e->cfg.shard_rank * kLineWords;
+  p.h_mmslot = mm_lines + (size_t)e->cfg.shard_rank * kLineWords;
   p.h_clist = e->cfg.shard_count > 1 ? e->shm_dev + shm_clist_offset_words() + (size_t)e->cfg.shard_rank * 2 * kCListWords : e->h_clist;
   p.topm = (batching && !getenv("KAI_NO_TOPM")) ? 1 : 0;
   p.scanners = e->lgrid;
@@ -1118,7 +1093,7 @@ int kai_engine_run(kai_engine *e, kai_action action, kai_result *out) {
     CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_record, kThreads, e->ltile_bytes));
     p.fused_in_kernel = (per_sm * e->num_sms >= e->lgrid && !getenv("KAI_NO_FUSED_LAUNCH")) ? 1 : 0;
   }
-  const unsigned int seq0 = e->seq;
+  const uint64_t seq0 = e->seq;
   CK(cudaMemsetAsync(e->counters, 0, sizeof(long long) * 48, e->stream));
   cudaEventRecord(e->ev[2], e->stream);
   if (e->J > 0) k_prep_jobs<<<std::min(e->num_sms * 8, (e->J + 255) / 256), 256, 0, e->stream>>>(e->ds, 1, 1);
@@ -1148,8 +1123,7 @@ int kai_engine_run(kai_engine *e, kai_action action, kai_result *out) {
   if (!engine_launch_record(e, load)) return e->cuda_fail(cudaGetLastError(), "k_record (tile load)");
   HostBackend &hb = e->hb;
   hb.h_slots = e->cfg.shard_count > 1 ? e->shm_base : e->h_slots;
-  hb.h_mm = e->cfg.shard_count > 1 ? e->shm_base + (size_t)2 * kMaxGrid * kSlotWords : e->h_mm;
-  hb.n_scanners = e->cfg.shard_count;  // the last CTA of every GPU reduces its scanners' answers: one line per GPU
+  hb.h_mm = e->cfg.shard_count > 1 ? e->shm_base + (size_t)2 * kShmRanks * kLineWords : e->h_mm;
   hb.topm = p.topm;
   hb.prof = getenv("KAI_PROFILE") != nullptr;
   for (int i = 0; i < 8; i++) hb.t_sec[i] = 0;
@@ -1170,6 +1144,7 @@ int kai_engine_run(kai_engine *e, kai_action action, kai_result *out) {
   hb.list_invalidate();
   hb.batching = batching;
   hb.failed = false;
+  hb.error_msg[0] = 0;
   hb.gang_fast = getenv("KAI_NO_GANG_FAST") == nullptr;
   hb.gang_bulk = hb.gang_replayed = hb.gang_failed = 0;
   hb.rank_to_node = e->rank_to_node_h.data();
@@ -1372,7 +1347,6 @@ int kai_engine_run(kai_engine *e, kai_action action, kai_result *out) {
   c[4] = seq.pods_evicted;
   c[5] = seq.minmax_exchanges;
   c[6] = seq.error;
-  c[7] = ctl.seq + 1;
   c[15] = seq.batched + hb.listed;
   if (hb.failed && c[24] == 0) c[24] = 99;
   // session state back to the device copies (later actions' prepare kernels and the result download read them)
@@ -1400,7 +1374,7 @@ int kai_engine_run(kai_engine *e, kai_action action, kai_result *out) {
   e->stats.nodes_scanned = c[2];
   e->stats.algorithmic_bytes = c[2] * ((2 * e->R + 1) * 8 + 4);
   e->stats.kernel_launches += e->record_launches + (e->J > 0) + (e->Q > 0);
-  e->seq = (unsigned int)c[7];
+  e->seq = ctl.seq;
   if (getenv("KAI_PROFILE")) {
     fprintf(stderr, "[kai] host-sequenced action %.3f ms, %lld sweeps, %lld batched placements, %lld minmax exchanges\n", ms, c[1], c[15], c[5]);
     fprintf(stderr, "[kai] host sequencer (%lld record launches): total %.3f ms, of which waiting for sweeps %.3f ms (%.2f us per sweep)\n",
@@ -1425,15 +1399,15 @@ int kai_engine_run(kai_engine *e, kai_action action, kai_result *out) {
   }
   if (c[24] != 0) {
     char msg[256];
-    snprintf(msg, sizeof(msg), "device protocol watchdog: wait code %lld seq %lld who %lld cta %lld (seq0 %u, end seq %lld)",
-             c[24], c[25], c[26], c[27], seq0, c[7]);
+    snprintf(msg, sizeof(msg), "device protocol watchdog: wait code %lld seq %lld who %lld cta %lld (seq0 %llu, end seq %llu)",
+             c[24], c[25], c[26], c[27], (unsigned long long)seq0, (unsigned long long)ctl.seq);
     e->loaded = false;
-    std::string m2 = msg;
+    std::string m2 = (c[24] == 99 && e->hb.error_msg[0]) ? std::string(e->hb.error_msg) : std::string(msg);
     char b2[96];
     m2 += "; host trace:";
     unsigned int n0 = e->hb.trace_n > 16 ? e->hb.trace_n - 16 : 0;
     for (unsigned int i = n0; i < e->hb.trace_n; i++) {
-      snprintf(b2, sizeof(b2), " (%u k%d nd%d)", e->hb.trace_seq[i & 63], e->hb.trace_kind[i & 63], e->hb.trace_nd[i & 63]);
+      snprintf(b2, sizeof(b2), " (%llu k%d nd%d)", e->hb.trace_seq[i & 63], e->hb.trace_kind[i & 63], e->hb.trace_nd[i & 63]);
       m2 += b2;
     }
     return e->fail(KAI_ERR_CUDA, m2);
@@ -1500,7 +1474,7 @@ int kai_engine_time_sweeps(kai_engine *e, int n_launches, double *elapsed_ms, do
   // the sweep kernel alone (its top-M lines stay in device memory), then the merge kernel alone on the last answer
   cudaEventRecord(e->ev[0], e->stream);
   for (int i = 0; i < n_launches; i++) {
-    rec.seq = e->seq + 1 + (unsigned int)i;
+    rec.seq = e->seq + (uint64_t)i;
     k_record<<<e->lgrid, kThreads, e->ltile_bytes, e->stream>>>(e->lp, rec);
   }
   cudaEventRecord(e->ev[1], e->stream);
@@ -1516,7 +1490,7 @@ int kai_engine_time_sweeps(kai_engine *e, int n_launches, double *elapsed_ms, do
   if (merge_ms) *merge_ms = ms;
   const int n_shard_rows = e->N > e->cfg.shard_rank ? (e->N - e->cfg.shard_rank + e->cfg.shard_count - 1) / e->cfg.shard_count : 0;
   *rows_per_launch = n_shard_rows;
-  e->seq += (unsigned int)n_launches + 4;
+  e->seq += (uint64_t)n_launches;
   return KAI_OK;
 }
 

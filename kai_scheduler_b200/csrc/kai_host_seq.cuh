@@ -3,7 +3,8 @@
 // A CPU thread of libkaigpu.so runs the sequencer (kai_seq.cuh) against a host mirror of the session state and sends
 // the GPU one decision record per node-table sweep: publish() = one k_record launch carrying the record in its kernel
 // parameters.  List answers come back as ONE merged, cut and sorted list per GPU (k_merge_cluster), single-row /
-// min-max answers as one line reduced by the last CTA; the host waits on a sequence tag in pinned host memory.
+// min-max answers as one line reduced by the last CTA; the host waits on the sequence number written last into the list
+// header or the line, in pinned host memory.
 //
 // Why: the pointer-chasing part of the cycle (heap pops, DRF keys, statement log) is a chain of dependent accesses per
 // job; a host core serves it from its caches far faster than one GPU lane (latencies in profiles/microbench).  The
@@ -11,6 +12,7 @@
 #pragma once
 #include <algorithm>
 #include <chrono>
+#include <cstdio>
 #include <cstring>
 #include <vector>
 
@@ -21,14 +23,16 @@
 namespace kai {
 
 struct HostBackend {
-  // pinned, device-mapped answer lines: one per GPU
-  unsigned long long *h_slots = nullptr;  // [2][kMaxGrid][kSlotWords]
-  unsigned long long *h_mm = nullptr;     // [2][kMaxGrid][kSlotWords]
-  int n_scanners = 0;
+  // pinned, device-mapped answer lines, one per GPU: [2][n_ranks][kLineWords], parity by sequence number.  Other ranks
+  // read a rank's lines, so one line per parity is not enough; two are: a rank issues answered record k + 2 only after
+  // every rank has answered k + 1, and each rank answers k + 1 only after it has read all lines of k (records that are
+  // not answered take no sequence number).
+  unsigned long long *h_slots = nullptr;
+  unsigned long long *h_mm = nullptr;
   int batching = 1;
   double timeout_s = 20.0;
   bool failed = false;
-  char error_msg[256] = {0};  // why the action failed, when the sequencer sets Seq::error to a code that carries a message
+  char error_msg[256] = {0};  // why the action failed: Seq::error codes that carry a message, an answer line that moved on
   const int *rank_to_node = nullptr;  // host copy
   Ctl ctl;
   Seq seq;
@@ -75,7 +79,7 @@ struct HostBackend {
   bool prof = false;
   unsigned long long t_sec[8] = {0, 0, 0, 0, 0, 0, 0, 0};  // rdtsc: pop, admit, place (incl. sweeps), finish, loop
   int trace_kind[64];
-  unsigned int trace_seq[64];
+  unsigned long long trace_seq[64];
   int trace_nd[64];
   unsigned int trace_n = 0;
   // ---- a record is a kernel launch (k_record), the answer one merged line / list per GPU ----
@@ -108,59 +112,63 @@ struct HostBackend {
     if (prof) t_launch += now() - tl;
   }
 
-  // gather the answer line of every GPU (written by its last CTA over PCIe as single 16-byte stores)
+  const unsigned long long *answer_line(const unsigned long long *lines, unsigned long long seq_no, int rank) const {
+    return lines + ((size_t)(seq_no & 1) * n_ranks + rank) * kLineWords;
+  }
+  // Wait for the line of record seq_no (its last word), copy the payload, then check that the line was not rewritten
+  // for a later record meanwhile; false (and the action fails) on a timeout or a changed line.
+  bool read_line(const unsigned long long *line, unsigned long long seq_no, unsigned long long *payload) {
+    unsigned long long v;
+    if (!wait_word(line + kLineWords - 1, [&](unsigned long long x) { return x == seq_no; }, v)) return false;
+    for (int i = 0; i < kLineWords - 1; i++) payload[i] = __atomic_load_n(line + i, __ATOMIC_RELAXED);
+    __atomic_thread_fence(__ATOMIC_ACQUIRE);  // the payload loads complete before the re-check
+    v = __atomic_load_n(line + kLineWords - 1, __ATOMIC_RELAXED);
+    if (v == seq_no) return true;
+    failed = true;
+    snprintf(error_msg, sizeof(error_msg), "answer line of record %llu changed to record %llu while it was read", seq_no, v);
+    return false;
+  }
+
+  // gather the answer line of every GPU (written by its last CTA over PCIe): {score, [flags:8][repeat:8][rank:24]}
+  // {cur_a gpu, cur_a cpu} {repeat tracker-event bits, -}
   void gather_candidates() {
-    const unsigned int seq_no = ctl.seq;
-    const unsigned long long *buf = h_slots + (size_t)(seq_no & 1) * kMaxGrid * kSlotWords;
-    const unsigned int tag = seq_no & 0xffffffu;
+    const unsigned long long seq_no = ctl.seq;
     double bs = -1.0;
-    uint32_t brank = kRankNone, bmeta = 0;
-    int bslot = -1;
-    for (int c = 0; c < n_scanners; c++) {
-      const unsigned long long *slot = buf + (size_t)c * kSlotWords;
-      unsigned long long hi;
-      if (!wait_word(slot + 1, [&](unsigned long long v) { return (unsigned int)(v >> 40) == tag; }, hi)) break;
-      unsigned long long lo = __atomic_load_n(slot, __ATOMIC_RELAXED);
+    uint32_t brank = kRankNone;
+    unsigned long long best[kLineWords - 1] = {0, 0, 0, 0, 0, 0, 0};
+    for (int r = 0; r < n_ranks; r++) {
+      unsigned long long w[kLineWords - 1];
+      if (!read_line(answer_line(h_slots, seq_no, r), seq_no, w)) break;
       double sc;
-      memcpy(&sc, &lo, 8);
-      uint32_t rk = (uint32_t)(hi & 0xffffffu);
+      memcpy(&sc, &w[0], 8);
+      uint32_t rk = (uint32_t)(w[1] & 0xffffffu);
       bool better_ = rk != kRankNone && (brank == kRankNone || sc > bs || (sc == bs && rk < brank));
       if (better_) {
         bs = sc;
         brank = rk;
-        bmeta = (uint32_t)((hi >> 24) & 0xffffu);
-        bslot = c;
+        memcpy(best, w, sizeof(best));
       }
     }
-    uint32_t bflags = bmeta >> 8, repeat = bmeta & 0xffu;
+    const uint32_t bflags = (uint32_t)((best[1] >> 32) & 0xffu), repeat = (uint32_t)((best[1] >> 24) & 0xffu);
     ctl.win.score = bs;
     ctl.win.rank = brank;
     ctl.win.flags = bflags;
     ctl.win.node = brank == kRankNone ? -1 : rank_to_node[brank];
     ctl.batch.valid = 0;
     if (brank != kRankNone && !failed) {
-      const unsigned long long *slot = buf + (size_t)bslot * kSlotWords;
       for (int k = 0; k < 2; k++) {
         uint32_t f = (bflags >> (3 * k)) & 7u;
         double a = 0;
-        if (f & WF_A_LT_MN) {
-          unsigned long long hi;
-          if (!wait_word(slot + 2 + 2 * k + 1, [&](unsigned long long v) { return (unsigned int)v == tag; }, hi)) break;
-          unsigned long long lo = __atomic_load_n(slot + 2 + 2 * k, __ATOMIC_RELAXED);
-          memcpy(&a, &lo, 8);
-        }
+        if (f & WF_A_LT_MN) memcpy(&a, &best[2 + k], 8);
         if (f) track_decrease(ctl.trk[k], f, a);
       }
       if (repeat) {
-        unsigned long long hi;
-        if (wait_word(slot + 7, [&](unsigned long long v) { return (unsigned int)v == tag; }, hi)) {
-          ctl.batch.valid = 1;
-          ctl.batch.node = ctl.win.node;
-          ctl.batch.to_idle = (bflags & SLOT_TO_IDLE) ? 1 : 0;
-          ctl.batch.left = (int)repeat;
-          ctl.batch.idx = 0;
-          ctl.batch.fl = __atomic_load_n(slot + 6, __ATOMIC_RELAXED);
-        }
+        ctl.batch.valid = 1;
+        ctl.batch.node = ctl.win.node;
+        ctl.batch.to_idle = (bflags & SLOT_TO_IDLE) ? 1 : 0;
+        ctl.batch.left = (int)repeat;
+        ctl.batch.idx = 0;
+        ctl.batch.fl = best[4];
       }
     }
     ctl.seq = seq_no + 1;
@@ -171,7 +179,7 @@ struct HostBackend {
   // order and mark the prefix that is provably the global order: entries strictly better than the last listed key of
   // any GPU that has more fitting rows than it listed.
   void gather_list() {
-    const unsigned int seq_no = ctl.seq;
+    const unsigned long long seq_no = ctl.seq;
     list.clear();
     bool have_cut = false;
     double cut_score = 0;
@@ -179,7 +187,7 @@ struct HostBackend {
     for (int r = 0; r < n_ranks && !failed; r++) {
       const unsigned long long *cl = h_clist + ((size_t)r * 2 + (seq_no & 1)) * kCListWords;
       unsigned long long hi;
-      if (!wait_word(cl + 1, [&](unsigned long long v) { return v == (unsigned long long)seq_no; }, hi)) break;
+      if (!wait_word(cl + 1, [&](unsigned long long v) { return v == seq_no; }, hi)) break;
       const unsigned long long head = __atomic_load_n(cl, __ATOMIC_RELAXED);
       const int n = (int)(head & 0x7fffffffu);
       const bool more = ((head >> 31) & 1ull) != 0;
@@ -404,20 +412,18 @@ struct HostBackend {
     return true;
   }
 
+  // the min/max line of every GPU: {gpu min, gpu max} {cpu min, cpu max} {gpu count at min | at max << 32, cpu counts}
   void gather_minmax() {
-    const unsigned int seq_no = ctl.seq;
-    const unsigned long long *buf = h_mm + (size_t)(seq_no & 1) * kMaxGrid * kSlotWords;
+    const unsigned long long seq_no = ctl.seq;
     double gmn[2] = {DBL_MAX, DBL_MAX}, gmx[2] = {0, 0};
     long long cmn[2] = {0, 0}, cmx[2] = {0, 0};
-    for (int c = 0; c < n_scanners && !failed; c++) {
-      const unsigned long long *slot = buf + (size_t)c * kSlotWords;
+    for (int r = 0; r < n_ranks && !failed; r++) {
+      unsigned long long w[kLineWords - 1];
+      if (!read_line(answer_line(h_mm, seq_no, r), seq_no, w)) break;
       for (int k = 0; k < 2; k++) {
-        unsigned long long hi, lo;
         double v;
-        if (!wait_word(slot + 4 * k + 1, [&](unsigned long long x) { return (x >> 32) == (unsigned long long)seq_no; }, hi)) break;
-        lo = __atomic_load_n(slot + 4 * k, __ATOMIC_RELAXED);
-        memcpy(&v, &lo, 8);
-        int cnt = (int)(hi & 0xffffffffu);
+        memcpy(&v, &w[2 * k], 8);
+        int cnt = (int)(w[4 + k] & 0xffffffffu);
         if (cnt > 0) {
           if (cmn[k] == 0 || v < gmn[k]) {
             gmn[k] = v;
@@ -425,10 +431,8 @@ struct HostBackend {
           } else if (v == gmn[k])
             cmn[k] += cnt;
         }
-        if (!wait_word(slot + 4 * k + 3, [&](unsigned long long x) { return (x >> 32) == (unsigned long long)seq_no; }, hi)) break;
-        lo = __atomic_load_n(slot + 4 * k + 2, __ATOMIC_RELAXED);
-        memcpy(&v, &lo, 8);
-        cnt = (int)(hi & 0xffffffffu);
+        memcpy(&v, &w[2 * k + 1], 8);
+        cnt = (int)(w[4 + k] >> 32);
         if (cnt > 0) {
           if (cmx[k] == 0 || v > gmx[k]) {
             gmx[k] = v;
@@ -595,8 +599,7 @@ struct HostBackend {
 
   void flush_deltas() {
     n_flush++;
-    publish(DK_FLUSH);  // stream order: the next launch sees these deltas applied; nothing to wait for
-    ctl.seq++;
+    publish(DK_FLUSH);  // stream order: the next launch sees these deltas applied; no answer, no sequence number
     ctl.n_delta = 0;
   }
 

@@ -77,7 +77,7 @@ enum { DB_GPU_TASK = 1, DB_BEST_EFFORT = 2, DB_PIPELINE_ONLY = 4, DB_BATCHING = 
 
 struct Ctl {  // sequencer control block
   int job, n_items, job_ok, item_ok, need_minmax, use_batch, stop;
-  unsigned int seq;  // sequence number of the next decision record
+  uint64_t seq;      // sequence number of the next answered record (SCAN, MINMAX, TOPK); it never restarts
   int n_delta;       // node deltas queued for the next record
   unsigned int xbits;  // XB_* bits of the next record
   unsigned int last_dkey;  // last queued delta: rank | code << 28, its first task and its repeat count
@@ -143,15 +143,15 @@ inline bool should_allocate(const Seq &q, int t, bool real) {  // pod_info.go:51
 
 void seq_flush_deltas(Seq &q);  // FLUSH record when the delta list is full (kai_host_seq.cuh)
 
-// Every delta word is written exactly once (readers validate it by its tag only): the newest entry stays pending in
+// Every delta word is written exactly once: the newest entry stays pending in
 // the control block, so that consecutive deltas of the same kind on the same row with bit-identical requests can be
-// folded into it as a repeat count (tag word bits 32+; the owner applies the same subtraction `count` times, in
+// folded into it as a repeat count (second word bits 32+; the owner applies the same subtraction `count` times, in
 // order).  close_delta() writes the pending entry; it is called before a record is published.
 inline void close_delta(Ctl &c, unsigned long long *delta_base) {
   if (c.n_delta > 0 && c.last_dcount > 0) {
     unsigned long long data = (unsigned long long)c.last_dkey | ((unsigned long long)(unsigned int)c.last_dtask << 32);
     store_tagged(delta_base + ((size_t)(c.seq & 1) * kMaxDelta + c.n_delta - 1) * 2, data,
-                 (unsigned long long)c.seq | ((unsigned long long)(c.last_dcount - 1) << 32));
+                 (unsigned long long)(c.last_dcount - 1) << 32);
   }
   c.last_dcount = 0;
 }

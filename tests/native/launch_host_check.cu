@@ -1,7 +1,9 @@
 // Host-only check of the launch transport's host side (kai_host_seq.cuh): (1) a decision record is packed into the
 // LaunchRec a k_record launch carries exactly as the scanners decode it (folded node deltas, repeat counts, extended
 // entries), (2) the merged candidate lists of several GPUs are merged with the cut rule applied across ranks, negative
-// and -0.0 scores included, (3) the integer sort key of k_merge_cluster orders every score as the comparator does.
+// and -0.0 scores included, (3) the integer sort key of k_merge_cluster orders every score as the comparator does,
+// (4) single-row and min-max answer lines are taken only under their full 64-bit sequence number, and a line that
+// changes while it is read fails the action.
 // Built and run by tests/test_launch_host.py (nvcc, no GPU needed: nothing is launched).
 #include <algorithm>
 #include <cfloat>
@@ -10,6 +12,10 @@
 #include <cstdlib>
 #include <cstring>
 #include <vector>
+
+#include <signal.h>
+#include <sys/mman.h>
+#include <unistd.h>
 
 #include "../../kai_scheduler_b200/csrc/kai_host_seq.cuh"
 
@@ -38,6 +44,118 @@ static bool fake_launch(void *, const LaunchRec &rec) {
       return 1;                     \
     }                               \
   } while (0)
+
+// ---------------------------------------------------------------- (4) answer lines
+// A line as the last CTA of k_record writes it: payload words, the sequence number in the last word.
+static void put_line(unsigned long long *line, const unsigned long long *payload, unsigned long long seq_no) {
+  for (int i = 0; i < kLineWords - 1; i++) line[i] = payload[i];
+  line[kLineWords - 1] = seq_no;
+}
+static unsigned long long dbits(double d) {
+  unsigned long long u;
+  memcpy(&u, &d, 8);
+  return u;
+}
+
+// A line whose number changes between the wait and the re-check: the payload sits at the end of a page that is not
+// readable yet, the sequence word at the start of the next page.  The wait sees the wanted number; the first payload
+// load faults, and the handler rewrites the sequence word (as the GPU would for a later record) and makes the payload
+// readable, so the re-check sees the new number.
+static unsigned long long *g_moving_seq = nullptr;
+static unsigned char *g_payload_page = nullptr;
+static size_t g_page = 0;
+static void move_on(int, siginfo_t *, void *) {
+  *g_moving_seq += 2;
+  mprotect(g_payload_page, g_page, PROT_READ | PROT_WRITE);
+}
+
+static int check_answer_lines(HostBackend &hb) {
+  std::vector<int> rank_to_node(64);
+  for (int i = 0; i < 64; i++) rank_to_node[i] = 1000 + i;
+  hb.rank_to_node = rank_to_node.data();
+  hb.failed = false;
+  hb.error_msg[0] = 0;
+  memset(&hb.ctl.trk, 0, sizeof(hb.ctl.trk));
+  for (int S = 1; S <= 3; S++) {
+    hb.n_ranks = S;
+    std::vector<unsigned long long> slots((size_t)2 * S * kLineWords, 0), mm((size_t)2 * S * kLineWords, 0);
+    hb.h_slots = slots.data();
+    hb.h_mm = mm.data();
+    // single-row lines above 2^32: rank r answers rank 10 + r with score 3 - r (rank 0 wins) and one repeat
+    const unsigned long long seq_no = (3ull << 32) + 17 + (unsigned long long)S;
+    for (int r = 0; r < S; r++) {
+      const unsigned long long meta = ((unsigned long long)SLOT_TO_IDLE << 32) | (1ull << 24) | (unsigned long long)(10 + r);
+      const unsigned long long w[kLineWords - 1] = {dbits(3.0 - r), meta, dbits(0.5), dbits(0.25), 0x2aull, 0, 0};
+      put_line(slots.data() + ((seq_no & 1) * S + r) * kLineWords, w, seq_no);
+    }
+    hb.ctl.seq = seq_no;
+    hb.gather_candidates();
+    CHECK(!hb.failed && hb.ctl.seq == seq_no + 1, "S=%d: single-row lines at seq %llu", S, seq_no);
+    CHECK(hb.ctl.win.score == 3.0 && hb.ctl.win.rank == 10 && hb.ctl.win.node == 1010 && hb.ctl.win.flags == SLOT_TO_IDLE,
+          "S=%d: winner score %g rank %u node %d flags %u", S, hb.ctl.win.score, hb.ctl.win.rank, hb.ctl.win.node, hb.ctl.win.flags);
+    CHECK(hb.ctl.batch.valid && hb.ctl.batch.left == 1 && hb.ctl.batch.node == 1010 && hb.ctl.batch.fl == 0x2aull, "S=%d: repeat", S);
+    // min/max lines above 2^32: rank r reports gpu [1 + r, 8 - r] with counts (r + 1, 2), cpu [5, 5] with (1, 1)
+    const unsigned long long mm_seq = seq_no + 1;
+    for (int r = 0; r < S; r++) {
+      const unsigned long long w[kLineWords - 1] = {dbits(1.0 + r), dbits(8.0 - r), dbits(5.0), dbits(5.0),
+                                                     (unsigned long long)(r + 1) | (2ull << 32), 1ull | (1ull << 32), 0};
+      put_line(mm.data() + ((mm_seq & 1) * S + r) * kLineWords, w, mm_seq);
+    }
+    hb.gather_minmax();
+    CHECK(!hb.failed && hb.ctl.seq == mm_seq + 1, "S=%d: min/max lines at seq %llu", S, mm_seq);
+    CHECK(hb.ctl.trk[0].mn == 1.0 && hb.ctl.trk[0].cnt_mn == 1 && hb.ctl.trk[0].mx == 8.0 && hb.ctl.trk[0].cnt_mx == 2,
+          "S=%d: gpu tracker %g x%d .. %g x%d", S, hb.ctl.trk[0].mn, hb.ctl.trk[0].cnt_mn, hb.ctl.trk[0].mx, hb.ctl.trk[0].cnt_mx);
+    CHECK(hb.ctl.trk[1].mn == 5.0 && hb.ctl.trk[1].cnt_mn == S && hb.ctl.trk[1].mx == 5.0 && hb.ctl.trk[1].cnt_mx == S,
+          "S=%d: cpu tracker", S);
+  }
+  // a stale line whose number agrees with the wanted one in its low 24 or low 32 bits is never taken
+  const double keep_timeout = hb.timeout_s;
+  hb.timeout_s = 0.05;
+  hb.n_ranks = 1;
+  const unsigned long long wanted = (1ull << 32) + (7ull << 24) + 12345;
+  const unsigned long long stale[2] = {wanted - (1ull << 24) * 2, wanted - (1ull << 32) * 2};  // same parity
+  for (int i = 0; i < 2; i++)
+    for (int kind = 0; kind < 2; kind++) {
+      std::vector<unsigned long long> lines((size_t)2 * kLineWords, 0);
+      const unsigned long long w[kLineWords - 1] = {dbits(1.0), 7ull, 0, 0, 0, 0, 0};
+      put_line(lines.data() + (wanted & 1) * kLineWords, w, stale[i]);
+      hb.h_slots = hb.h_mm = lines.data();
+      hb.failed = false;
+      hb.ctl.seq = wanted;
+      if (kind == 0)
+        hb.gather_candidates();
+      else
+        hb.gather_minmax();
+      CHECK(hb.failed && (kind == 1 || hb.ctl.win.node == -1), "stale line %llu taken for %llu (%s)", stale[i], wanted,
+            kind == 0 ? "single row" : "min/max");
+    }
+  hb.timeout_s = keep_timeout;
+  // a line that moves on to a later record between the wait and the re-check fails the action and names the record
+  g_page = (size_t)sysconf(_SC_PAGESIZE);
+  unsigned char *pages = (unsigned char *)mmap(nullptr, 2 * g_page, PROT_READ | PROT_WRITE, MAP_PRIVATE | MAP_ANONYMOUS, -1, 0);
+  CHECK(pages != MAP_FAILED, "mmap");
+  unsigned long long *line = (unsigned long long *)(pages + g_page) - (kLineWords - 1);
+  const unsigned long long w[kLineWords - 1] = {dbits(2.0), 3ull, 0, 0, 0, 0, 0};
+  const unsigned long long moving = 4242;
+  put_line(line, w, moving);
+  g_moving_seq = line + kLineWords - 1;
+  g_payload_page = pages;
+  struct sigaction sa, old;
+  memset(&sa, 0, sizeof(sa));
+  sa.sa_sigaction = &move_on;
+  sa.sa_flags = SA_SIGINFO;
+  sigaction(SIGSEGV, &sa, &old);
+  mprotect(pages, g_page, PROT_NONE);
+  unsigned long long payload[kLineWords - 1];
+  hb.failed = false;
+  hb.error_msg[0] = 0;
+  const bool ok = hb.read_line(line, moving, payload);
+  sigaction(SIGSEGV, &old, nullptr);
+  CHECK(!ok && hb.failed && *g_moving_seq == moving + 2, "a line that changed while it was read was accepted");
+  CHECK(strstr(hb.error_msg, "record 4242") != nullptr, "error message names the record: %s", hb.error_msg);
+  munmap(pages, 2 * g_page);
+  return 0;
+}
 
 int main() {
   // ---------------------------------------------------------------- (1) record packing
@@ -111,21 +229,31 @@ int main() {
   hb.ctl.xbits = XB_SINGLE;
   hb.publish(DK_SCAN);
   CHECK(g_launches == 1, "one launch per record, got %d", g_launches);
-  CHECK(g_last.seq == 7u && g_last.n_delta == (int)want.size(), "seq %u n_delta %d (want %zu)", g_last.seq, g_last.n_delta, want.size());
+  CHECK(g_last.seq == 7u && g_last.n_delta == (int)want.size(), "seq %llu n_delta %d (want %zu)", (unsigned long long)g_last.seq,
+        g_last.n_delta, want.size());
   CHECK((int)(g_last.dw[0] & 0xff) == DK_SCAN && (int)((g_last.dw[0] >> 32) & 0xffff) == (int)want.size(), "record word 0");
   CHECK(((unsigned int)(g_last.dw[0] >> 48) & XB_SINGLE) != 0, "xbits");
   for (size_t e = 0; e < want.size(); e++)
     CHECK(g_last.dkey[e] == want[e].key && g_last.dtask[e] == want[e].task && (int)g_last.dcount[e] == want[e].count - 1,
           "delta %zu: key %08x task %u count-1 %d, want %08x %u %d", e, g_last.dkey[e], g_last.dtask[e], (int)g_last.dcount[e], want[e].key,
           want[e].task, want[e].count - 1);
-  // a full list flushes by a launch of its own and the sequence number moves on without waiting
+  // a full list flushes by a launch of its own, without waiting and without taking a sequence number
   hb.ctl.seq = 8;
   hb.ctl.n_delta = 0;
   hb.ctl.last_dcount = 0;
   for (int i = 0; i < kMaxDelta + 3; i++) emit_delta(hb.seq, i % N, ND_ADD, (i * 5) % T);  // neighbours differ: no folding
   CHECK(g_launches == 2 && (int)(g_last.dw[0] & 0xff) == DK_FLUSH && g_last.n_delta == kMaxDelta, "flush launch: %d launches, kind %d, n_delta %d",
         g_launches, (int)(g_last.dw[0] & 0xff), g_last.n_delta);
-  CHECK(hb.ctl.seq == 9u && hb.ctl.n_delta == 3, "after the flush: seq %u n_delta %d", hb.ctl.seq, hb.ctl.n_delta);
+  CHECK(g_last.seq == 8u && hb.ctl.seq == 8u && hb.ctl.n_delta == 3, "after the flush: record seq %llu, next seq %llu, n_delta %d",
+        (unsigned long long)g_last.seq, (unsigned long long)hb.ctl.seq, hb.ctl.n_delta);
+  // past 2^32 the record still carries the whole number, and the folded repeat counts are intact
+  hb.ctl.seq = (5ull << 32) + 9;
+  hb.ctl.n_delta = 0;
+  hb.ctl.last_dcount = 0;
+  for (int t = 0; t < 4; t++) emit_delta(hb.seq, 5, ND_ADD, t);
+  hb.publish(DK_SCAN);
+  CHECK(g_last.seq == (5ull << 32) + 9 && g_last.n_delta == 1 && g_last.dcount[0] == 3, "record at seq 2^32 * 5 + 9: seq %llu n_delta %d count-1 %d",
+        (unsigned long long)g_last.seq, g_last.n_delta, (int)g_last.dcount[0]);
 
   // ---------------------------------------------------------------- (2) merging the GPUs' lists
   for (int trial = 0; trial < 200; trial++) {
@@ -134,7 +262,7 @@ int main() {
     hb.h_clist = clist.data();
     hb.n_ranks = S;
     hb.failed = false;
-    const unsigned int seq_no = 100 + (unsigned int)trial;
+    const unsigned long long seq_no = 100 + (unsigned long long)trial;
     hb.ctl.seq = seq_no;
     struct Ent {
       double score;
@@ -252,8 +380,10 @@ int main() {
       for (int i = 0; i < n; i++) CHECK(list_key(c[i].v) < ~0ull, "key trial %d: %a reaches the empty slot", trial, c[i].v);
       pairs += n;
     }
-    printf("OK record packing (%zu deltas, flush), 200 multi-GPU list merges and the list sort key (%lld candidates)\n",
+    printf("OK record packing (%zu deltas, flush), 200 multi-GPU list merges and the list sort key (%lld candidates)",
            want.size(), pairs);
   }
+  if (int rc = check_answer_lines(hb)) return rc;
+  printf(", answer lines\n");
   return 0;
 }

@@ -394,21 +394,3 @@ def test_structural_edit_under_the_same_epoch_is_refused():
     finally:
         e.close()
     assert len(checked) == len(rl.STRUCTURAL_FIELDS) - 1
-
-
-# ---------------------------------------------------------------- sequence reset
-
-def test_sequence_reset_on_resident_loads(monkeypatch):
-    """KAI_SEQ_RESET_AT lowers the threshold of the sequence-number restart so that resident cycles cross it many
-    times; every action must still equal the oracle."""
-    monkeypatch.setenv("KAI_SEQ_RESET_AT", "300")
-    rng = np.random.default_rng(21)
-    snap = synthetic.reclaim_snapshot(n_nodes=48, running_per_node=7, victim_queues=2, reclaimer_jobs=12, reclaimer_tasks=2,
-                                      reclaimer_gpus=3.0)
-    loads, resident = run_cycles(rl.prepare(snap, rng), rng, abi.make_config(**FUZZ_CFG), cycles=10, what="reset",
-                                 full_every=4)
-    assert (loads, resident) == (10, 7)
-    for seed in range(5):
-        rng = np.random.default_rng(9500 + seed)
-        snap = rl.prepare(dsl.build_snapshot(_random_topology(rng))[0], rng)
-        run_cycles(snap, rng, abi.make_config(**FUZZ_CFG), cycles=10, what=f"reset seed {seed}", full_every=4)

@@ -5,6 +5,8 @@ filter's top-k list when the rows it needs are known from the mirror, from its n
 against the oracle:
   * "default":  the default maximum (small sets on the host, the rest on the GPU);
   * "gpu":      KAI_HOST_SWEEP_MAX=0, every sweep on the GPU (the path before host answers existed);
+  * "gpu-split": as "gpu", with KAI_NO_FUSED_LAUNCH=1: a sweep's binpack extremes come from a MINMAX launch followed by
+                the sweep launch instead of the exchange inside one cooperative launch;
   * "check":    every eligible sweep and top-k list answered on the host AND on the GPU (KAI_HOST_SWEEP_CHECK=1),
                 the action fails on any difference (node, score bits, name rank, flags; the listed rows).
 """
@@ -22,6 +24,7 @@ pytestmark = pytest.mark.gpu
 MODES = {
     "default": {},
     "gpu": {"KAI_HOST_SWEEP_MAX": "0"},
+    "gpu-split": {"KAI_HOST_SWEEP_MAX": "0", "KAI_NO_FUSED_LAUNCH": "1"},
     "check": {"KAI_HOST_SWEEP_MAX": "100000000", "KAI_HOST_SWEEP_CHECK": "1"},
 }
 
@@ -30,6 +33,7 @@ MODES = {
 def sweep_mode(request, monkeypatch):
     monkeypatch.delenv("KAI_HOST_SWEEP_MAX", raising=False)
     monkeypatch.delenv("KAI_HOST_SWEEP_CHECK", raising=False)
+    monkeypatch.delenv("KAI_NO_FUSED_LAUNCH", raising=False)
     for k, v in MODES[request.param].items():
         monkeypatch.setenv(k, v)
     return request.param
