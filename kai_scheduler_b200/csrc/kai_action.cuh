@@ -182,8 +182,9 @@ struct Cand {
   uint32_t rank;
   int ln;
 };
-// better / binpack_score / node_key are compiled for the host too: the solver answers small restricted sweeps from its
-// node mirror with the very operations the scanners run (kadd & co. are IEEE binary64 without contraction on both sides)
+// better / binpack_score / row_fits / row_score / node_key / repeat_row are compiled for the host too: the solver answers
+// small restricted sweeps from its node mirror with the very operations the scanners run (kadd & co. are IEEE binary64
+// without contraction on both sides)
 KAI_HD __forceinline__ bool better(double sa, uint32_t ra, double sb, uint32_t rb) {
   if (ra == kRankNone) return false;
   if (rb == kRankNone) return true;
@@ -202,192 +203,201 @@ KAI_HD __forceinline__ double binpack_score(double mn, double mx, double cur, do
   return kmul(9.0, t4);
 }
 
-// FittingNode (session.go:201-232) + NodeOrderFn sum (session_plugins.go:427-437) of one node row given as
-// Idle/Releasing vectors.  Returns false if the node does not fit; fit_i = fits on Idle alone.
-KAI_HD __forceinline__ bool node_key(const Decision &d, int R, const double *I, const double *L, int stride,
-                                     double a_gpu, double a_cpu, double gpu_count, uint32_t nflags, int n,
-                                     double &score, bool &fit_i) {
+// The rules below take a node row as Idle/Releasing vectors with resource r at [r * stride].  They only ever index it
+// with constants after unrolling, so a row held in registers (stride 1) stays in registers.
+//
+// FittingNode (session.go:201-232) of request rq[R]: returns whether the row fits on Idle + Releasing; fit_i = fits on
+// Idle alone.
+KAI_HD __forceinline__ bool row_fits(const double *rq, int R, const double *I, const double *L, int stride, bool &fit_i) {
   bool fit_ri = true;
   fit_i = true;
-  for (int r = 0; r < R; r++) {
+  KAI_UNROLL
+  for (int r = 0; r < KAI_MAX_RES; r++) {
+    if (r >= R) break;
     double i = I[r * stride];
     double avail = kadd(i, L[r * stride]);
-    double rq = d.req[r];
     if (r >= 3) {
-      if (rq != 0 && rq > avail) fit_ri = false;
-      if (rq != 0 && rq > i) fit_i = false;
+      if (rq[r] != 0 && rq[r] > avail) fit_ri = false;
+      if (rq[r] != 0 && rq[r] > i) fit_i = false;
     } else {
-      if (rq > avail) fit_ri = false;
-      if (rq > i) fit_i = false;
+      if (rq[r] > avail) fit_ri = false;
+      if (rq[r] > i) fit_i = false;
     }
   }
-  if (!fit_ri) return false;
-  score = 0.0;
+  return fit_ri;
+}
+
+// NodeOrderFn sum (session_plugins.go:427-437) of node n's row, in the reference's operation order
+KAI_HD __forceinline__ double row_score(const Decision &d, const double *I, const double *L, int stride, double a_gpu,
+                                        double a_cpu, double gpu_count, uint32_t nflags, int n, bool fit_i) {
+  double score = 0.0;
   score = kadd(score, (d.best_effort || fit_i) ? 100.0 : 0.0);  // nodeavailability.go:29-40
   score = kadd(score, 0.0);                                   // gpusharingorder (whole GPUs)
   bool cpu_only_node = !(nflags & KAI_NODE_NOT_CPU_ONLY) && a_gpu <= 0;
   score = kadd(score, (!d.gpu_task && cpu_only_node) ? 10.0 : 0.0);  // resourcetype.go:29-41
   score = kadd(score, (d.nominated == n) ? 1000000.0 : 0.0);        // nominatednode.go:29-41
-  double cur = kadd(I[d.res * stride], L[d.res * stride]);
-  double overall = d.res == KAI_RES_GPU ? a_gpu : a_cpu;
+  const bool gpu = d.res == KAI_RES_GPU;  // the scored resource is GPU or CPU
+  double cur = gpu ? kadd(I[KAI_RES_GPU * stride], L[KAI_RES_GPU * stride]) : kadd(I[KAI_RES_CPU * stride], L[KAI_RES_CPU * stride]);
+  double overall = gpu ? a_gpu : a_cpu;
   double place;
   if (d.strategy == KAI_PLACEMENT_BINPACK) {
     place = binpack_score(d.mn, d.mx, cur, overall);
   } else {  // spread.go:16-36
-    double cnt = d.res == KAI_RES_GPU ? (double)(long long)gpu_count : overall;
+    double cnt = gpu ? (double)(long long)gpu_count : overall;
     place = cnt == 0 ? 0.0 : kdiv(cur, cnt);
   }
-  score = kadd(score, place);
+  return kadd(score, place);
+}
+
+// FittingNode + NodeOrderFn of node n's row.  Returns false if the node does not fit; fit_i = fits on Idle alone.
+KAI_HD __forceinline__ bool node_key(const Decision &d, int R, const double *I, const double *L, int stride,
+                                     double a_gpu, double a_cpu, double gpu_count, uint32_t nflags, int n,
+                                     double &score, bool &fit_i) {
+  if (!row_fits(d.req, R, I, L, stride, fit_i)) return false;
+  score = row_score(d, I, L, stride, a_gpu, a_cpu, gpu_count, nflags, n, fit_i);
   return true;
 }
 
-// The sweep over this CTA's tile followed by the block argmax on (score desc, name rank asc).
-__device__ Cand scan_tile(const Tile &tl, const Decision &d, const DevSnap &s, Cand *sh_warp,
-                          const int *excl = nullptr, int n_excl = 0, int *fit_count = nullptr, int xbits = 0,
-                          int pref_level = -1, const unsigned char *dom_bucket = nullptr) {
-  Cand best;
-  int n_fit = 0;
-  best.score = -1.0;
-  best.rank = kRankNone;
-  best.ln = -1;
-  const uint32_t *mask = d.pred_class >= 0 ? s.pred_mask + (size_t)d.pred_class * s.mask_words : nullptr;
-  const uint32_t dom_need = dom_need_mask((unsigned int)xbits);
-  for (int ln = threadIdx.x; ln < tl.count; ln += blockDim.x) {
-    int n = tl.node[ln];
-    if (d.restricted && !(tl.flags[ln] & kTileFeas)) continue;
-    if ((xbits & XB_RESTRICT_DOM) && (tl.flags[ln] & dom_need) != dom_need) continue;
-    if (mask && !((__ldg(&mask[n >> 5]) >> (n & 31)) & 1u)) continue;
-    double score;
-    bool fit_i;
-    if (!node_key(d, tl.R, tl.I + ln, tl.L + ln, tl.npc, tl.Agpu[ln], tl.Acpu[ln], tl.gpu_count[ln], tl.flags[ln], n,
-                  score, fit_i))
-      continue;
-    if (pref_level >= 0) {  // topology/node_scoring.go:17-53, the last NodeOrderFn of the default tiers
-      const int dd = tl.dom[pref_level * tl.npc + ln];
-      const unsigned char bk = (dd >= 0 && dd < kDomBuckets) ? dom_bucket[dd] : (unsigned char)255;
-      if (bk == 255) continue;  // no entry: NodeOrderFn fails, the node is dropped (session.go:247-251)
-      score = __dadd_rn(score, __dmul_rn((double)bk, 10000.0));
+// Same-node repeats (DESIGN.md §5): row ln of the tile after k placements of d's request, in registers.  The mode is
+// decided on the row before any placement (common/allocate.go:165-174); the placements subtract the request in order,
+// with the f64 operations of the sequential application (node_info.go:457-493).  Returns whether placement k may repeat
+// the winning placement: the row still fits (`fits`), in the same mode, and its score plus the row's topology term
+// `topo` is at least the winning score `win`, so node ln stays the argmax.
+KAI_HD __forceinline__ bool repeat_row(const Tile &tl, const Decision &d, int ln, int k, double win, double topo,
+                                       double (&I)[KAI_MAX_RES], double (&L)[KAI_MAX_RES], bool &to_idle, bool &fits) {
+  const int R = tl.R;
+  double rq[KAI_MAX_RES];
+  KAI_UNROLL
+  for (int r = 0; r < KAI_MAX_RES; r++) {
+    I[r] = r < R ? tl.I[r * tl.npc + ln] : 0.0;
+    L[r] = r < R ? tl.L[r * tl.npc + ln] : 0.0;
+    rq[r] = r < R ? d.req[r] : 0.0;
+  }
+  bool fit_i;
+  row_fits(rq, R, I, L, 1, fit_i);
+  to_idle = !d.pipeline_only && (d.best_effort || fit_i);
+  for (int j = 0; j < k; j++) {
+    KAI_UNROLL
+    for (int r = 0; r < KAI_MAX_RES; r++) {
+      if (to_idle)
+        I[r] = ksub(I[r], rq[r]);  // rq[r] = 0 beyond R: exact no-op
+      else
+        L[r] = ksub(L[r], rq[r]);
     }
+  }
+  fits = row_fits(rq, R, I, L, 1, fit_i);
+  if (!fits) return false;
+  const double sc = row_score(d, I, L, 1, tl.Agpu[ln], tl.Acpu[ln], tl.gpu_count[ln], tl.flags[ln], tl.node[ln], fit_i);
+  return (!d.pipeline_only && (d.best_effort || fit_i)) == to_idle && kadd(sc, topo) >= win;
+}
+
+// The sweeps' row set: the restricted feasible set and the selected topology domains
+__device__ __forceinline__ bool in_row_set(const Tile &tl, int ln, bool restricted, int xbits) {
+  if (restricted && !(tl.flags[ln] & kTileFeas)) return false;
+  const uint32_t need = dom_need_mask((unsigned int)xbits);
+  return !(xbits & XB_RESTRICT_DOM) || (tl.flags[ln] & need) == need;
+}
+
+// argmax on (score desc, name rank asc) over the lanes of a warp: the winner on lane 0
+__device__ __forceinline__ Cand warp_argmax(Cand c) {
+  for (int o = 16; o > 0; o >>= 1) {
+    Cand x;
+    x.score = __shfl_down_sync(0xffffffffu, c.score, o);
+    x.rank = __shfl_down_sync(0xffffffffu, c.rank, o);
+    x.ln = __shfl_down_sync(0xffffffffu, c.ln, o);
+    if (better(x.score, x.rank, c.score, c.rank)) c = x;
+  }
+  return c;
+}
+
+// The sweep over this CTA's tile followed by the block argmax on (score desc, name rank asc).  key(ln, score) is the rule
+// of the sweep: false when row ln is not a candidate, else its score.  Candidates in excl[0, n_excl) are counted but not
+// taken; fit_count (if set) receives the number of candidates.
+template <class Key>
+__device__ Cand scan_tile(const Tile &tl, Key key, Cand *sh_warp, const int *excl, int n_excl, int *fit_count) {
+  Cand best = {-1.0, kRankNone, -1};
+  int n_fit = 0;
+  for (int ln = threadIdx.x; ln < tl.count; ln += blockDim.x) {
+    double score;
+    if (!key(ln, score)) continue;
     n_fit++;
     bool skip = false;
     for (int x = 0; x < n_excl; x++)
       if (excl[x] == ln) skip = true;
     if (skip) continue;
     uint32_t rk = (uint32_t)tl.rank[ln];
-    if (better(score, rk, best.score, best.rank)) {
-      best.score = score;
-      best.rank = rk;
-      best.ln = ln;
-    }
+    if (better(score, rk, best.score, best.rank)) best = {score, rk, ln};
   }
   if (fit_count) {
     int w = __reduce_add_sync(0xffffffffu, n_fit);
     if ((threadIdx.x & 31) == 0 && w) atomicAdd(fit_count, w);
   }
-  for (int o = 16; o > 0; o >>= 1) {
-    double os = __shfl_down_sync(0xffffffffu, best.score, o);
-    uint32_t orank = __shfl_down_sync(0xffffffffu, best.rank, o);
-    int oln = __shfl_down_sync(0xffffffffu, best.ln, o);
-    if (better(os, orank, best.score, best.rank)) {
-      best.score = os;
-      best.rank = orank;
-      best.ln = oln;
-    }
-  }
+  best = warp_argmax(best);
   int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (lane == 0) sh_warp[warp] = best;
   __syncthreads();
   if (warp == 0) {
-    int nw = blockDim.x >> 5;
-    Cand c;
-    if (lane < nw)
-      c = sh_warp[lane];
-    else {
-      c.score = -1.0;
-      c.rank = kRankNone;
-      c.ln = -1;
-    }
-    for (int o = 16; o > 0; o >>= 1) {
-      double os = __shfl_down_sync(0xffffffffu, c.score, o);
-      uint32_t orank = __shfl_down_sync(0xffffffffu, c.rank, o);
-      int oln = __shfl_down_sync(0xffffffffu, c.ln, o);
-      if (better(os, orank, c.score, c.rank)) {
-        c.score = os;
-        c.rank = orank;
-        c.ln = oln;
-      }
-    }
-    best = c;
+    Cand c = {-1.0, kRankNone, -1};
+    if (lane < (int)(blockDim.x >> 5)) c = sh_warp[lane];
+    best = warp_argmax(c);
   }
   return best;  // valid on thread 0
 }
 
-// Block argmax on (idle + releasing GPUs desc, name rank asc) over the rows strictly after the cutoff.
-__device__ Cand scan_tile_topk(const Tile &tl, const Decision &d, Cand *sh_warp, const int *excl, int n_excl,
-                               int *fit_count) {
-  Cand best;
-  int n_fit = 0;
-  best.score = -1.0;
-  best.rank = kRankNone;
-  best.ln = -1;
-  const bool has_cut = d.req[2] != 0.0;
-  const double cut_key = d.req[0];
-  const uint32_t cut_rank = (uint32_t)d.req[1];
-  for (int ln = threadIdx.x; ln < tl.count; ln += blockDim.x) {
-    double key = __dadd_rn(tl.I[KAI_RES_GPU * tl.npc + ln], tl.L[KAI_RES_GPU * tl.npc + ln]);
-    uint32_t rk = (uint32_t)tl.rank[ln];
-    if (has_cut && !(key < cut_key || (key == cut_key && rk > cut_rank))) continue;
-    n_fit++;
-    bool skip = false;
-    for (int x = 0; x < n_excl; x++)
-      if (excl[x] == ln) skip = true;
-    if (skip) continue;
-    if (better(key, rk, best.score, best.rank)) {
-      best.score = key;
-      best.rank = rk;
-      best.ln = ln;
-    }
-  }
-  if (fit_count) {
-    int w = __reduce_add_sync(0xffffffffu, n_fit);
-    if ((threadIdx.x & 31) == 0 && w) atomicAdd(fit_count, w);
-  }
-  for (int o = 16; o > 0; o >>= 1) {
-    double os = __shfl_down_sync(0xffffffffu, best.score, o);
-    uint32_t orank = __shfl_down_sync(0xffffffffu, best.rank, o);
-    int oln = __shfl_down_sync(0xffffffffu, best.ln, o);
-    if (better(os, orank, best.score, best.rank)) {
-      best.score = os;
-      best.rank = orank;
-      best.ln = oln;
-    }
-  }
-  int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (lane == 0) sh_warp[warp] = best;
+// The kTopM best candidates of this CTA in key order into cands (a missing one has rank kRankNone; excl lists their rows),
+// and the number of candidates into *fit_count
+template <class Key>
+__device__ void scan_top_m(const Tile &tl, Key key, Cand *sh_warp, int *excl, Cand *cands, int *fit_count) {
+  if (threadIdx.x == 0) *fit_count = 0;
   __syncthreads();
-  if (warp == 0) {
-    int nw = blockDim.x >> 5;
-    Cand c;
-    if (lane < nw)
-      c = sh_warp[lane];
-    else {
-      c.score = -1.0;
-      c.rank = kRankNone;
-      c.ln = -1;
+  for (int m = 0; m < kTopM; m++) {
+    Cand c = scan_tile(tl, key, sh_warp, excl, m, m == 0 ? fit_count : nullptr);
+    if (threadIdx.x == 0) {
+      cands[m] = c;
+      excl[m] = c.ln;
     }
-    for (int o = 16; o > 0; o >>= 1) {
-      double os = __shfl_down_sync(0xffffffffu, c.score, o);
-      uint32_t orank = __shfl_down_sync(0xffffffffu, c.rank, o);
-      int oln = __shfl_down_sync(0xffffffffu, c.ln, o);
-      if (better(os, orank, c.score, c.rank)) {
-        c.score = os;
-        c.rank = orank;
-        c.ln = oln;
-      }
-    }
-    best = c;
+    __syncthreads();
   }
-  return best;  // valid on thread 0
+}
+
+// pack.go:66-86 over this CTA's rows of the row set (the predicate mask does not apply): min and max of Idle + Releasing
+// of GPU (k = 0) and CPU (k = 1) over the rows whose Allocatable of that resource is not 0, folded over the block
+// through sh_d (4 per warp).  Every thread returns the CTA's extremes.
+__device__ void tile_extremes(const Tile &tl, bool restricted, int xbits, double *sh_d, double (&mn)[2], double (&mx)[2]) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+  mn[0] = mn[1] = DBL_MAX;
+  mx[0] = mx[1] = 0.0;
+  for (int ln = threadIdx.x; ln < tl.count; ln += blockDim.x) {
+    if (!in_row_set(tl, ln, restricted, xbits)) continue;
+    for (int k = 0; k < 2; k++) {
+      int res = k == 0 ? KAI_RES_GPU : KAI_RES_CPU;
+      double overall = k == 0 ? tl.Agpu[ln] : tl.Acpu[ln];
+      if (overall == 0) continue;
+      double cur = __dadd_rn(tl.I[res * tl.npc + ln], tl.L[res * tl.npc + ln]);
+      if (cur < mn[k]) mn[k] = cur;
+      if (cur > mx[k]) mx[k] = cur;
+    }
+  }
+  for (int k = 0; k < 2; k++)
+    for (int o = 16; o > 0; o >>= 1) {
+      mn[k] = fmin(mn[k], __shfl_xor_sync(0xffffffffu, mn[k], o));
+      mx[k] = fmax(mx[k], __shfl_xor_sync(0xffffffffu, mx[k], o));
+    }
+  if (lane == 0) {
+    sh_d[warp * 4 + 0] = mn[0];
+    sh_d[warp * 4 + 1] = mx[0];
+    sh_d[warp * 4 + 2] = mn[1];
+    sh_d[warp * 4 + 3] = mx[1];
+  }
+  __syncthreads();
+  for (int k = 0; k < 2; k++) {
+    mn[k] = DBL_MAX;
+    mx[k] = 0.0;
+    for (int w = 0; w < nw; w++) {
+      mn[k] = fmin(mn[k], sh_d[w * 4 + 2 * k]);
+      mx[k] = fmax(mx[k], sh_d[w * 4 + 2 * k + 1]);
+    }
+  }
 }
 
 // answer slot of a scanner in xbuf (8 x u64), read by the last CTA of the same launch after the ticket:
@@ -400,9 +410,8 @@ constexpr int kSlotWords = 8;
 // (i = 0 is the swept placement, i >= 1 are candidate repeats on the same node); lane 0 then walks the
 // placements in order to simulate the min/max trackers and decides how many repeats it can vouch for.
 __device__ void publish_candidate(const Track *trk, const Tile &tl, const Decision &d, Cand local,
-                                  unsigned long long *slot, int batching, long long *dbg = nullptr) {
+                                  unsigned long long *slot, int batching) {
   const int lane = threadIdx.x & 31;
-  long long d0 = clock64(), d1 = d0, d2 = d0, d3 = d0;
   local.score = __shfl_sync(0xffffffffu, local.score, 0);
   local.rank = __shfl_sync(0xffffffffu, local.rank, 0);
   local.ln = __shfl_sync(0xffffffffu, local.ln, 0);
@@ -410,80 +419,17 @@ __device__ void publish_candidate(const Track *trk, const Tile &tl, const Decisi
   double a_gpu = 0, a_cpu = 0;
   unsigned long long rep_flags = 0;
   if (local.rank != kRankNone) {  // warp-uniform
-    const int ln = local.ln, R = tl.R, n = tl.node[ln];
-    // the row lives in registers: every index below is a compile-time constant after unrolling
-    double I[KAI_MAX_RES], L[KAI_MAX_RES], rq[KAI_MAX_RES];
-#pragma unroll
-    for (int r = 0; r < KAI_MAX_RES; r++) {
-      I[r] = r < R ? tl.I[r * tl.npc + ln] : 0.0;
-      L[r] = r < R ? tl.L[r * tl.npc + ln] : 0.0;
-      rq[r] = r < R ? d.req[r] : 0.0;
-    }
-    const double ag = tl.Agpu[ln], ac = tl.Acpu[ln], gc = tl.gpu_count[ln];
-    const uint32_t nf = tl.flags[ln];
-    bool fit_i0 = true;
-#pragma unroll
-    for (int r = 0; r < KAI_MAX_RES; r++)
-      if (r < R && (r >= 3 ? (rq[r] != 0 && rq[r] > I[r]) : (rq[r] > I[r]))) fit_i0 = false;
-    const bool to_idle = !d.pipeline_only && (d.best_effort || fit_i0);  // common/allocate.go:165-174
-    // state before placement `lane`: the row after `lane` placements (node_info.go:457-493), same f64 ops
-    // in the same order as the sequential application
-    const int me = lane <= kMaxRepeat ? lane : kMaxRepeat;
-    for (int k = 0; k < me; k++) {
-#pragma unroll
-      for (int r = 0; r < KAI_MAX_RES; r++) {
-        if (to_idle)
-          I[r] = __dsub_rn(I[r], rq[r]);  // rq[r] = 0 beyond R: exact no-op
-        else
-          L[r] = __dsub_rn(L[r], rq[r]);
-      }
-    }
-    d1 = clock64();
-    bool ok = true;  // placement `lane` is admissible as a repeat
-    if (lane > 0) {
-      // FittingNode + NodeOrderFn on the register row (same operations as node_key)
-      bool fit_ri = true, fi = true;
-#pragma unroll
-      for (int r = 0; r < KAI_MAX_RES; r++) {
-        if (r >= R) continue;
-        double avail = __dadd_rn(I[r], L[r]);
-        if (r >= 3) {
-          if (rq[r] != 0 && rq[r] > avail) fit_ri = false;
-          if (rq[r] != 0 && rq[r] > I[r]) fi = false;
-        } else {
-          if (rq[r] > avail) fit_ri = false;
-          if (rq[r] > I[r]) fi = false;
-        }
-      }
-      if (!fit_ri)
-        ok = false;
-      else {
-        double sc = 0.0;
-        sc = __dadd_rn(sc, (d.best_effort || fi) ? 100.0 : 0.0);
-        sc = __dadd_rn(sc, 0.0);
-        bool cpu_only_node = !(nf & KAI_NODE_NOT_CPU_ONLY) && ag <= 0;
-        sc = __dadd_rn(sc, (!d.gpu_task && cpu_only_node) ? 10.0 : 0.0);
-        sc = __dadd_rn(sc, (d.nominated == n) ? 1000000.0 : 0.0);
-        double cur = d.res == KAI_RES_GPU ? __dadd_rn(I[KAI_RES_GPU], L[KAI_RES_GPU]) : __dadd_rn(I[KAI_RES_CPU], L[KAI_RES_CPU]);
-        double overall = d.res == KAI_RES_GPU ? ag : ac;
-        double place;
-        if (d.strategy == KAI_PLACEMENT_BINPACK) {
-          place = binpack_score(d.mn, d.mx, cur, overall);
-        } else {
-          double cnt = d.res == KAI_RES_GPU ? (double)(long long)gc : overall;
-          place = cnt == 0 ? 0.0 : __ddiv_rn(cur, cnt);
-        }
-        sc = __dadd_rn(sc, place);
-        bool ti = !d.pipeline_only && (d.best_effort || fi);
-        if (ti != to_idle) ok = false;
-        if (!(sc >= local.score)) ok = false;  // node n must stay the argmax (DESIGN.md §5)
-      }
-    }
+    const int ln = local.ln;
+    double I[KAI_MAX_RES], L[KAI_MAX_RES];
+    bool to_idle, fits;
+    // topology term 0: the repeat's score without it against the swept score with it finds fewer repeats, never a wrong one
+    bool ok = repeat_row(tl, d, ln, lane <= kMaxRepeat ? lane : kMaxRepeat, local.score, 0.0, I, L, to_idle, fits);
+    const double ag = tl.Agpu[ln], ac = tl.Acpu[ln];
     double b2[2] = {0, 0}, a2[2] = {0, 0};
     int has[2] = {0, 0};
     {
       const double Ig = I[KAI_RES_GPU], Lg = L[KAI_RES_GPU], Ic = I[KAI_RES_CPU], Lc = L[KAI_RES_CPU];
-      const double rg = rq[KAI_RES_GPU], rc = rq[KAI_RES_CPU];
+      const double rg = d.req[KAI_RES_GPU], rc = d.req[KAI_RES_CPU];
       if (ag != 0 && rg != 0) {
         has[0] = 1;
         b2[0] = __dadd_rn(Ig, Lg);
@@ -495,7 +441,6 @@ __device__ void publish_candidate(const Track *trk, const Tile &tl, const Decisi
         a2[1] = to_idle ? __dadd_rn(__dsub_rn(Ic, rc), Lc) : __dadd_rn(Ic, __dsub_rn(Lc, rc));
       }
     }
-    d2 = clock64();
     // Tracker events of placement `lane`.  Within a batch min/max of both resources are constant (the batch
     // ends before any placement that would move them), so every lane can evaluate its events against the
     // trackers of the record; only the "last node leaves the max" rule needs a prefix count.
@@ -548,14 +493,8 @@ __device__ void publish_candidate(const Track *trk, const Tile &tl, const Decisi
       rep_flags = ((unsigned long long)hi32 << 32) | lo32;
     }
     if (repeat) flags |= SLOT_HAS_REPEAT;
-    d3 = clock64();
   }
   if (lane != 0) return;
-  if (dbg) {
-    dbg[0] += d1 - d0;
-    dbg[1] += d2 - d1;
-    dbg[2] += d3 - d2;
-  }
   st_relaxed_b128(slot + 2, (unsigned long long)__double_as_longlong(a_gpu), (unsigned long long)__double_as_longlong(a_cpu));
   if (repeat) st_relaxed_b128(slot + 4, rep_flags, 0ull);
   unsigned long long meta = ((unsigned long long)(flags & 0xffu) << 32) | ((unsigned long long)(repeat & 0xffu) << 24) |
@@ -572,81 +511,25 @@ __device__ void publish_candidate(const Track *trk, const Tile &tl, const Decisi
 // ---------------------------------------------------------------------------------------------
 enum { LF_TO_IDLE = 1, LF_EXHAUSTED = 2, LF_MORE = 4, LF_HAS_GPU = 8, LF_HAS_CPU = 16 };
 __device__ void publish_list_candidate(const Tile &tl, const Decision &d, Cand c, bool more, unsigned long long *line0_word,
-                                       unsigned long long *payload_line, double topo_term = 0.0) {
+                                       unsigned long long *payload_line, double topo_term) {
   const int lane = threadIdx.x & 31;
   uint32_t flags = more ? LF_MORE : 0u, repeat = 0;
   double Ig0 = 0, Lg0 = 0, Ic0 = 0, Lc0 = 0;
   if (c.rank != kRankNone) {  // warp-uniform
-    const int ln = c.ln, R = tl.R, n = tl.node[ln];
-    double I[KAI_MAX_RES], L[KAI_MAX_RES], rq[KAI_MAX_RES];
-#pragma unroll
-    for (int r = 0; r < KAI_MAX_RES; r++) {
-      I[r] = r < R ? tl.I[r * tl.npc + ln] : 0.0;
-      L[r] = r < R ? tl.L[r * tl.npc + ln] : 0.0;
-      rq[r] = r < R ? d.req[r] : 0.0;
-    }
-    Ig0 = I[KAI_RES_GPU];
-    Lg0 = L[KAI_RES_GPU];
-    Ic0 = I[KAI_RES_CPU];
-    Lc0 = L[KAI_RES_CPU];
-    const double ag = tl.Agpu[ln], ac = tl.Acpu[ln], gc = tl.gpu_count[ln];
-    const uint32_t nf = tl.flags[ln];
-    if (ag != 0 && rq[KAI_RES_GPU] != 0) flags |= LF_HAS_GPU;
-    if (ac != 0 && rq[KAI_RES_CPU] != 0) flags |= LF_HAS_CPU;
-    bool fit_i0 = true;
-#pragma unroll
-    for (int r = 0; r < KAI_MAX_RES; r++)
-      if (r < R && (r >= 3 ? (rq[r] != 0 && rq[r] > I[r]) : (rq[r] > I[r]))) fit_i0 = false;
-    const bool to_idle = !d.pipeline_only && (d.best_effort || fit_i0);
+    const int ln = c.ln;
+    Ig0 = tl.I[KAI_RES_GPU * tl.npc + ln];
+    Lg0 = tl.L[KAI_RES_GPU * tl.npc + ln];
+    Ic0 = tl.I[KAI_RES_CPU * tl.npc + ln];
+    Lc0 = tl.L[KAI_RES_CPU * tl.npc + ln];
+    if (tl.Agpu[ln] != 0 && d.req[KAI_RES_GPU] != 0) flags |= LF_HAS_GPU;
+    if (tl.Acpu[ln] != 0 && d.req[KAI_RES_CPU] != 0) flags |= LF_HAS_CPU;
+    double I[KAI_MAX_RES], L[KAI_MAX_RES];
+    bool to_idle, fits;
+    // the row's topology score is the same for every repeat
+    const bool ok = repeat_row(tl, d, ln, lane <= kMaxRepeat + 1 ? lane : kMaxRepeat + 1, c.score, topo_term, I, L, to_idle, fits);
     if (to_idle) flags |= LF_TO_IDLE;
-    const int me = lane <= kMaxRepeat + 1 ? lane : kMaxRepeat + 1;  // row after `me` placements
-    for (int k = 0; k < me; k++) {
-#pragma unroll
-      for (int r = 0; r < KAI_MAX_RES; r++) {
-        if (to_idle)
-          I[r] = __dsub_rn(I[r], rq[r]);
-        else
-          L[r] = __dsub_rn(L[r], rq[r]);
-      }
-    }
-    bool fit_ri = true, fi = true;
-#pragma unroll
-    for (int r = 0; r < KAI_MAX_RES; r++) {
-      if (r >= R) continue;
-      double avail = __dadd_rn(I[r], L[r]);
-      if (r >= 3) {
-        if (rq[r] != 0 && rq[r] > avail) fit_ri = false;
-        if (rq[r] != 0 && rq[r] > I[r]) fi = false;
-      } else {
-        if (rq[r] > avail) fit_ri = false;
-        if (rq[r] > I[r]) fi = false;
-      }
-    }
-    bool ok = fit_ri;
-    if (ok) {
-      double sc = 0.0;
-      sc = __dadd_rn(sc, (d.best_effort || fi) ? 100.0 : 0.0);
-      sc = __dadd_rn(sc, 0.0);
-      bool cpu_only_node = !(nf & KAI_NODE_NOT_CPU_ONLY) && ag <= 0;
-      sc = __dadd_rn(sc, (!d.gpu_task && cpu_only_node) ? 10.0 : 0.0);
-      sc = __dadd_rn(sc, (d.nominated == n) ? 1000000.0 : 0.0);
-      double cur = d.res == KAI_RES_GPU ? __dadd_rn(I[KAI_RES_GPU], L[KAI_RES_GPU]) : __dadd_rn(I[KAI_RES_CPU], L[KAI_RES_CPU]);
-      double overall = d.res == KAI_RES_GPU ? ag : ac;
-      double place;
-      if (d.strategy == KAI_PLACEMENT_BINPACK) {
-        place = binpack_score(d.mn, d.mx, cur, overall);
-      } else {
-        double cnt = d.res == KAI_RES_GPU ? (double)(long long)gc : overall;
-        place = cnt == 0 ? 0.0 : __ddiv_rn(cur, cnt);
-      }
-      sc = __dadd_rn(sc, place);
-      sc = __dadd_rn(sc, topo_term);  // the row's topology score is the same for every repeat
-      bool ti = !d.pipeline_only && (d.best_effort || fi);
-      if (ti != to_idle) ok = false;
-      if (!(sc >= c.score)) ok = false;
-    }
     const unsigned ok_mask = __ballot_sync(0xffffffffu, ok);
-    const unsigned fit_mask = __ballot_sync(0xffffffffu, fit_ri);
+    const unsigned fit_mask = __ballot_sync(0xffffffffu, fits);
     int r_n = 0;
     for (int i2 = 1; i2 <= kMaxRepeat; i2++) {
       if (!((ok_mask >> i2) & 1u)) break;
@@ -947,36 +830,13 @@ __device__ bool scanner_main(const ActionParams &p, const LaunchRec *lrec, unsig
     } else if (kind == DK_SCAN && (sh.xbits & XB_FUSED_MM)) {
       {
         // pack.go:66-86 over the current node set: local extremes -> device slots -> every scanner reduces all slots
-        double mn[2] = {DBL_MAX, DBL_MAX}, mx[2] = {0, 0};
-        for (int ln = tid; ln < tile.count; ln += blockDim.x)
-          for (int k = 0; k < 2; k++) {
-            int res = k == 0 ? KAI_RES_GPU : KAI_RES_CPU;
-            double overall = k == 0 ? tile.Agpu[ln] : tile.Acpu[ln];
-            if (overall == 0) continue;
-            if (sh.dec.restricted && !(tile.flags[ln] & kTileFeas)) continue;
-            if ((sh.xbits & XB_RESTRICT_DOM) && (tile.flags[ln] & dom_need_mask((unsigned int)sh.xbits)) != dom_need_mask((unsigned int)sh.xbits)) continue;
-            double cur = __dadd_rn(tile.I[res * tile.npc + ln], tile.L[res * tile.npc + ln]);
-            if (cur < mn[k]) mn[k] = cur;
-            if (cur > mx[k]) mx[k] = cur;
-          }
-        for (int k = 0; k < 2; k++)
-          for (int o = 16; o > 0; o >>= 1) {
-            mn[k] = fmin(mn[k], __shfl_xor_sync(0xffffffffu, mn[k], o));
-            mx[k] = fmax(mx[k], __shfl_xor_sync(0xffffffffu, mx[k], o));
-          }
-        if (lane == 0) {
-          sh_d[warp * 4 + 0] = mn[0];
-          sh_d[warp * 4 + 1] = mx[0];
-          sh_d[warp * 4 + 2] = mn[1];
-          sh_d[warp * 4 + 3] = mx[1];
-        }
-        __syncthreads();
+        double mn[2], mx[2];
+        tile_extremes(tile, sh.dec.restricted, sh.xbits, sh_d, mn, mx);
         // the one wait inside a launch: every scanner's extremes, tagged with the full sequence number (a slot of an
         // earlier record never matches), under the watchdog so that a protocol bug ends the kernel
         unsigned long long *mmbase = p.mmbuf;
         if (tid < 4) {
-          double v = tid & 1 ? 0.0 : DBL_MAX;
-          for (int w = 0; w < nw; w++) v = tid & 1 ? fmax(v, sh_d[w * 4 + tid]) : fmin(v, sh_d[w * 4 + tid]);
+          const double v = tid == 0 ? mn[0] : tid == 1 ? mx[0] : tid == 2 ? mn[1] : mx[1];
           st_relaxed_b128(mmbase + (size_t)my * kSlotWords + 2 * tid, (unsigned long long)__double_as_longlong(v),
                           seq);
         }
@@ -1011,18 +871,29 @@ __device__ bool scanner_main(const ActionParams &p, const LaunchRec *lrec, unsig
         __syncthreads();
       }
     }
+    // the placement sweep's key of a row: row set, predicate mask, FittingNode + NodeOrderFn, topology term
+    const Decision &dec = sh.dec;
+    const uint32_t *mask = dec.pred_class >= 0 ? s.pred_mask + (size_t)dec.pred_class * s.mask_words : nullptr;
+    const int xbits = sh.xbits, pref_level = sh.pref_level;
+    auto place_key = [&](int ln, double &score) {
+      const int n = tile.node[ln];
+      if (!in_row_set(tile, ln, dec.restricted, xbits)) return false;
+      if (mask && !((__ldg(&mask[n >> 5]) >> (n & 31)) & 1u)) return false;
+      bool fit_i;
+      if (!node_key(dec, tile.R, tile.I + ln, tile.L + ln, tile.npc, tile.Agpu[ln], tile.Acpu[ln], tile.gpu_count[ln],
+                    tile.flags[ln], n, score, fit_i))
+        return false;
+      if (pref_level >= 0) {  // topology/node_scoring.go:17-53, the last NodeOrderFn of the default tiers
+        const int dd = tile.dom[pref_level * tile.npc + ln];
+        const unsigned char bk = (dd >= 0 && dd < kDomBuckets) ? sh.dom_bucket[dd] : (unsigned char)255;
+        if (bk == 255) return false;  // no entry: NodeOrderFn fails, the node is dropped (session.go:247-251)
+        score = __dadd_rn(score, __dmul_rn((double)bk, 10000.0));
+      }
+      return true;
+    };
     if (kind == DK_SCAN && p.topm && !(sh.xbits & XB_SINGLE)) {
       // ---- top-M answer into device lines (k_merge_cluster merges them; no last-CTA reduction) ----
-      if (tid == 0) sh.fit_count = 0;
-      __syncthreads();
-      for (int m = 0; m < kTopM; m++) {
-        Cand c = scan_tile(tile, sh.dec, s, sh_warp, sh.excl, m, m == 0 ? &sh.fit_count : nullptr, sh.xbits, sh.pref_level, sh.dom_bucket);
-        if (tid == 0) {
-          sh.cands[m] = c;
-          sh.excl[m] = c.ln;
-        }
-        __syncthreads();
-      }
+      scan_top_m(tile, place_key, sh_warp, sh.excl, sh.cands, &sh.fit_count);
       if (tid == 0) ts[4] += clock64() - c3;
       unsigned long long *lines = p.d_list + (size_t)my * kListLines * kListLineWords;
       if (warp < kTopM) {
@@ -1037,16 +908,15 @@ __device__ bool scanner_main(const ActionParams &p, const LaunchRec *lrec, unsig
     } else if (kind == DK_TOPK) {
       // ---- accumulated_scenario_filters/idle_gpus: rows by idle + releasing GPUs, descending (name rank ascending
       //      among equals), strictly after the cutoff (req[0] = key, req[1] = rank, req[2] = cutoff present) ----
-      if (tid == 0) sh.fit_count = 0;
-      __syncthreads();
-      for (int m = 0; m < kTopM; m++) {
-        Cand c = scan_tile_topk(tile, sh.dec, sh_warp, sh.excl, m, m == 0 ? &sh.fit_count : nullptr);
-        if (tid == 0) {
-          sh.cands[m] = c;
-          sh.excl[m] = c.ln;
-        }
-        __syncthreads();
-      }
+      const bool has_cut = dec.req[2] != 0.0;
+      const double cut_key = dec.req[0];
+      const uint32_t cut_rank = (uint32_t)dec.req[1];
+      auto idle_gpu_key = [&](int ln, double &key) {
+        key = __dadd_rn(tile.I[KAI_RES_GPU * tile.npc + ln], tile.L[KAI_RES_GPU * tile.npc + ln]);
+        const uint32_t rk = (uint32_t)tile.rank[ln];
+        return !has_cut || key < cut_key || (key == cut_key && rk > cut_rank);
+      };
+      scan_top_m(tile, idle_gpu_key, sh_warp, sh.excl, sh.cands, &sh.fit_count);
       unsigned long long *lines = p.d_list + (size_t)my * kListLines * kListLineWords;
       if (tid < kTopM) {
         const Cand c = sh.cands[tid];
@@ -1055,49 +925,20 @@ __device__ bool scanner_main(const ActionParams &p, const LaunchRec *lrec, unsig
         st_relaxed_sys_b128(lines + 2 * tid, (unsigned long long)__double_as_longlong(c.score), hi);
       }
     } else if (kind == DK_SCAN) {
-      Cand local = scan_tile(tile, sh.dec, s, sh_warp, nullptr, 0, nullptr, sh.xbits, sh.pref_level, sh.dom_bucket);
+      Cand local = scan_tile(tile, place_key, sh_warp, nullptr, 0, nullptr);
       long long c4 = clock64();
       if (tid == 0) ts[4] += c4 - c3;
-      if (warp == 0) publish_candidate(sh.trk, tile, sh.dec, local, slot, sh.batching, my == 0 ? p.counters + 40 : nullptr);
+      if (warp == 0) publish_candidate(sh.trk, tile, sh.dec, local, slot, sh.batching);
     } else if (kind == DK_MINMAX) {
-      double mn[2] = {DBL_MAX, DBL_MAX}, mx[2] = {0, 0};
-      for (int ln = tid; ln < tile.count; ln += blockDim.x)
-        for (int k = 0; k < 2; k++) {
-          int res = k == 0 ? KAI_RES_GPU : KAI_RES_CPU;
-          double overall = k == 0 ? tile.Agpu[ln] : tile.Acpu[ln];
-          if (overall == 0) continue;
-          if (sh.dec.restricted && !(tile.flags[ln] & kTileFeas)) continue;
-          if ((sh.xbits & XB_RESTRICT_DOM) && (tile.flags[ln] & dom_need_mask((unsigned int)sh.xbits)) != dom_need_mask((unsigned int)sh.xbits)) continue;
-          double cur = __dadd_rn(tile.I[res * tile.npc + ln], tile.L[res * tile.npc + ln]);
-          if (cur < mn[k]) mn[k] = cur;
-          if (cur > mx[k]) mx[k] = cur;
-        }
-      for (int k = 0; k < 2; k++)
-        for (int o = 16; o > 0; o >>= 1) {
-          mn[k] = fmin(mn[k], __shfl_xor_sync(0xffffffffu, mn[k], o));
-          mx[k] = fmax(mx[k], __shfl_xor_sync(0xffffffffu, mx[k], o));
-        }
-      if (lane == 0) {
-        sh_d[warp * 4 + 0] = mn[0];
-        sh_d[warp * 4 + 1] = mx[0];
-        sh_d[warp * 4 + 2] = mn[1];
-        sh_d[warp * 4 + 3] = mx[1];
-      }
-      __syncthreads();
-      for (int w = 0; w < nw; w++) {
-        mn[0] = fmin(mn[0], sh_d[w * 4 + 0]);
-        mx[0] = fmax(mx[0], sh_d[w * 4 + 1]);
-        mn[1] = fmin(mn[1], sh_d[w * 4 + 2]);
-        mx[1] = fmax(mx[1], sh_d[w * 4 + 3]);
-      }
+      double mn[2], mx[2];
+      tile_extremes(tile, dec.restricted, xbits, sh_d, mn, mx);
       int c[4] = {0, 0, 0, 0};
       for (int ln = tid; ln < tile.count; ln += blockDim.x)
         for (int k = 0; k < 2; k++) {
           int res = k == 0 ? KAI_RES_GPU : KAI_RES_CPU;
           double overall = k == 0 ? tile.Agpu[ln] : tile.Acpu[ln];
           if (overall == 0) continue;
-          if (sh.dec.restricted && !(tile.flags[ln] & kTileFeas)) continue;
-          if ((sh.xbits & XB_RESTRICT_DOM) && (tile.flags[ln] & dom_need_mask((unsigned int)sh.xbits)) != dom_need_mask((unsigned int)sh.xbits)) continue;
+          if (!in_row_set(tile, ln, dec.restricted, xbits)) continue;
           double cur = __dadd_rn(tile.I[res * tile.npc + ln], tile.L[res * tile.npc + ln]);
           if (cur == mn[k]) c[2 * k]++;
           if (cur == mx[k]) c[2 * k + 1]++;
@@ -1158,41 +999,24 @@ __device__ void reduce_answers(const ActionParams &p, int kind, unsigned long lo
   const unsigned long long *buf = p.xbuf;
   unsigned long long *out = (kind == DK_SCAN ? p.h_slot : p.h_mmslot) + (size_t)(seq & 1) * p.cfg.shard_count * kLineWords;
   if (kind == DK_SCAN) {
-    double bs = -1.0;
-    uint32_t brank = kRankNone;
-    unsigned long long bmeta = (unsigned long long)kRankNone;
-    int bslot = -1;
+    Cand best = {-1.0, kRankNone, -1};  // ln: the winner's slot
     for (int c = lane; c < n; c += 32) {
       unsigned long long lo, hi;
       ld_relaxed_b128(buf + (size_t)c * kSlotWords, lo, hi);
       double sc = __longlong_as_double((long long)lo);
       uint32_t rk = (uint32_t)(hi & 0xffffffu);
-      if (better(sc, rk, bs, brank)) {
-        bs = sc;
-        brank = rk;
-        bmeta = hi;
-        bslot = c;
-      }
+      if (better(sc, rk, best.score, best.rank)) best = {sc, rk, c};
     }
-    for (int o = 16; o > 0; o >>= 1) {
-      double os = __shfl_xor_sync(0xffffffffu, bs, o);
-      uint32_t orank = __shfl_xor_sync(0xffffffffu, brank, o);
-      unsigned long long ometa = __shfl_xor_sync(0xffffffffu, bmeta, o);
-      int osl = __shfl_xor_sync(0xffffffffu, bslot, o);
-      if (better(os, orank, bs, brank)) {
-        bs = os;
-        brank = orank;
-        bmeta = ometa;
-        bslot = osl;
+    best = warp_argmax(best);
+    if (lane == 0) {  // the winning slot's meta word, cur_a values and repeat events
+      unsigned long long meta = (unsigned long long)kRankNone, ag = 0, ac = 0, rep = 0, unused;
+      if (best.rank != kRankNone) {
+        const unsigned long long *slot = buf + (size_t)best.ln * kSlotWords;
+        ld_relaxed_b128(slot, unused, meta);
+        ld_relaxed_b128(slot + 2, ag, ac);
+        if ((meta >> 24) & 0xffu) ld_relaxed_b128(slot + 4, rep, unused);
       }
-    }
-    if (lane == 0) {  // the winning slot's cur_a values and repeat events
-      unsigned long long ag = 0, ac = 0, rep = 0, unused;
-      if (brank != kRankNone) {
-        ld_relaxed_b128(buf + (size_t)bslot * kSlotWords + 2, ag, ac);
-        if ((bmeta >> 24) & 0xffu) ld_relaxed_b128(buf + (size_t)bslot * kSlotWords + 4, rep, unused);
-      }
-      st_relaxed_sys_b128(out, (unsigned long long)__double_as_longlong(bs), bmeta);
+      st_relaxed_sys_b128(out, (unsigned long long)__double_as_longlong(best.score), meta);
       st_relaxed_sys_b128(out + 2, ag, ac);
       st_relaxed_sys_b128(out + 4, rep, 0ull);
     }
@@ -1204,25 +1028,9 @@ __device__ void reduce_answers(const ActionParams &p, int kind, unsigned long lo
       for (int k = 0; k < 2; k++) {
         unsigned long long lo, hi;
         ld_relaxed_b128(slot + 4 * k, lo, hi);
-        double v = __longlong_as_double((long long)lo);
-        int cnt = (int)(hi & 0xffffffffu);
-        if (cnt > 0) {
-          if (cmn[k] == 0 || v < gmn[k]) {
-            gmn[k] = v;
-            cmn[k] = cnt;
-          } else if (v == gmn[k])
-            cmn[k] += cnt;
-        }
+        merge_extreme(gmn[k], cmn[k], __longlong_as_double((long long)lo), (int)(hi & 0xffffffffu), true);
         ld_relaxed_b128(slot + 4 * k + 2, lo, hi);
-        v = __longlong_as_double((long long)lo);
-        cnt = (int)(hi & 0xffffffffu);
-        if (cnt > 0) {
-          if (cmx[k] == 0 || v > gmx[k]) {
-            gmx[k] = v;
-            cmx[k] = cnt;
-          } else if (v == gmx[k])
-            cmx[k] += cnt;
-        }
+        merge_extreme(gmx[k], cmx[k], __longlong_as_double((long long)lo), (int)(hi & 0xffffffffu), false);
       }
     }
     for (int k = 0; k < 2; k++)
@@ -1231,20 +1039,8 @@ __device__ void reduce_answers(const ActionParams &p, int kind, unsigned long lo
         long long ocmn = __shfl_xor_sync(0xffffffffu, cmn[k], o);
         double omx = __shfl_xor_sync(0xffffffffu, gmx[k], o);
         long long ocmx = __shfl_xor_sync(0xffffffffu, cmx[k], o);
-        if (ocmn > 0) {
-          if (cmn[k] == 0 || omn < gmn[k]) {
-            gmn[k] = omn;
-            cmn[k] = ocmn;
-          } else if (omn == gmn[k])
-            cmn[k] += ocmn;
-        }
-        if (ocmx > 0) {
-          if (cmx[k] == 0 || omx > gmx[k]) {
-            gmx[k] = omx;
-            cmx[k] = ocmx;
-          } else if (omx == gmx[k])
-            cmx[k] += ocmx;
-        }
+        merge_extreme(gmn[k], cmn[k], omn, ocmn, true);
+        merge_extreme(gmx[k], cmx[k], omx, ocmx, false);
       }
     if (lane == 0) {
       unsigned long long cnt[2];

@@ -41,6 +41,12 @@ constexpr int kAllocatedStatuses = KAI_POD_ALLOCATED | KAI_POD_BOUND | KAI_POD_B
 // shared by the kernels and the host sequencer
 // ---------------------------------------------------------------------------------------------
 #define KAI_HD __host__ __device__
+// full unrolling in device code of shared functions (the host compiler does not know the pragma)
+#ifdef __CUDA_ARCH__
+#define KAI_UNROLL _Pragma("unroll")
+#else
+#define KAI_UNROLL
+#endif
 
 // IEEE binary64 without contraction on both sides
 KAI_HD inline double kadd(double a, double b) {
@@ -107,6 +113,17 @@ struct Track {  // global min/max of NonAllocated(res) over nodes with Allocatab
   int cnt_mn, cnt_mx;
   int dirty;
 };
+// Merge of two partial binpack extremes (pack.go:66-86) given as (value, number of rows at it): (v, cnt) into (m, c).
+// `lower` merges minima, else maxima; a side without rows (count 0) carries no value.
+KAI_HD inline void merge_extreme(double &m, long long &c, double v, long long cnt, bool lower) {
+  if (cnt <= 0) return;
+  if (c == 0 || (lower ? v < m : v > m)) {
+    m = v;
+    c = cnt;
+  } else if (v == m) {
+    c += cnt;
+  }
+}
 // tracker event bits per resource (gpu bits 0-2, cpu bits 3-5)
 enum { WF_B_EQ_MX = 1, WF_A_EQ_MN = 2, WF_A_LT_MN = 4 };
 KAI_HD inline uint32_t track_flags(const Track &t, double b, double a) {

@@ -1393,9 +1393,6 @@ int kai_engine_run(kai_engine *e, kai_action action, kai_result *out) {
     if (c[38] > 0)
       fprintf(stderr, "[kai] scanner 0 per record (cycles): record words %lld, decode %lld, deltas %lld, scan %lld, scan+publish %lld\n",
               c[33] / c[38], c[34] / c[38], c[35] / c[38], c[36] / c[38], c[37] / c[38]);
-    if (c[38] > 0)
-      fprintf(stderr, "[kai] publish_candidate of scanner 0 (cycles per record): row+advance %lld, key %lld, events+pack %lld\n",
-              c[40] / c[38], c[41] / c[38], c[42] / c[38]);
   }
   if (c[24] != 0) {
     char msg[256];

@@ -423,23 +423,9 @@ struct HostBackend {
       for (int k = 0; k < 2; k++) {
         double v;
         memcpy(&v, &w[2 * k], 8);
-        int cnt = (int)(w[4 + k] & 0xffffffffu);
-        if (cnt > 0) {
-          if (cmn[k] == 0 || v < gmn[k]) {
-            gmn[k] = v;
-            cmn[k] = cnt;
-          } else if (v == gmn[k])
-            cmn[k] += cnt;
-        }
+        merge_extreme(gmn[k], cmn[k], v, (int)(w[4 + k] & 0xffffffffu), true);
         memcpy(&v, &w[2 * k + 1], 8);
-        cnt = (int)(w[4 + k] >> 32);
-        if (cnt > 0) {
-          if (cmx[k] == 0 || v > gmx[k]) {
-            gmx[k] = v;
-            cmx[k] = cnt;
-          } else if (v == gmx[k])
-            cmx[k] += cnt;
-        }
+        merge_extreme(gmx[k], cmx[k], v, (int)(w[4 + k] >> 32), false);
       }
     }
     for (int k = 0; k < 2; k++) {  // pack.go:66-86: min starts at MaxFloat64, max at 0

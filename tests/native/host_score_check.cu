@@ -1,8 +1,11 @@
-// Host build of the scanners' scoring (kai_action.cuh: node_key, binpack_score, better), the code the solver also runs
-// on the host to answer small restricted sweeps from its node mirror.  Reads one case per line on stdin and prints the
-// result, so tests/test_host_score.py can compare it bit for bit with the oracle's scoring:
+// Host build of the scanners' scoring (kai_action.cuh: node_key, repeat_row, binpack_score, better), the code the solver
+// also runs on the host to answer small restricted sweeps from its node mirror.  Reads one case per line on stdin and
+// prints the result, so tests/test_host_score.py can compare it bit for bit with the oracle's scoring:
 //   K R strategy res gpu_task best_effort nominated n mn mx a_gpu a_cpu gpu_count nflags req[R] I[R] L[R]
 //       -> "K <fits> <fit_i> <score as %a>"
+//   A R ... (as K) ... L[R] pipeline_only k win
+//       -> "A <to_idle> <repeat ok> <fits> <fit_i> <score as %a>": repeat_row's row after k placements (no topology term),
+//          then row_fits / row_score on it
 //   P mn mx cur overall      -> "P <binpack_score as %a>"
 //   B sa ra sb rb            -> "B <better(sa, ra, sb, rb)>"
 // Doubles are read with strtod (hexadecimal floats are exact).  No GPU is needed: nothing is launched.
@@ -40,9 +43,10 @@ int main() {
       printf("P %a\n", binpack_score(D(1), D(2), D(3), D(4)));
     } else if (f[0] == "B") {
       printf("B %d\n", better(D(1), (uint32_t)I(2), D(3), (uint32_t)I(4)) ? 1 : 0);
-    } else if (f[0] == "K") {
+    } else if (f[0] == "K" || f[0] == "A") {
+      const bool adv = f[0] == "A";
       const int R = (int)I(1);
-      if (R < 1 || R > KAI_MAX_RES || f.size() != 14 + 3 * (size_t)R) {
+      if (R < 1 || R > KAI_MAX_RES || f.size() != 14 + 3 * (size_t)R + (adv ? 3 : 0)) {
         printf("FAIL bad case line\n");
         return 1;
       }
@@ -56,8 +60,8 @@ int main() {
       const int n = (int)I(7);
       d.mn = D(8);
       d.mx = D(9);
-      const double a_gpu = D(10), a_cpu = D(11), gpu_count = D(12);
-      const uint32_t nflags = (uint32_t)I(13);
+      double a_gpu = D(10), a_cpu = D(11), gpu_count = D(12);
+      uint32_t nflags = (uint32_t)I(13);
       std::vector<double> row(2 * R);
       for (int r = 0; r < R; r++) {
         d.req[r] = D(14 + r);
@@ -66,8 +70,32 @@ int main() {
       }
       double score = 0;
       bool fit_i = false;
-      const bool fits = node_key(d, R, row.data(), row.data() + R, 1, a_gpu, a_cpu, gpu_count, nflags, n, score, fit_i);
-      printf("K %d %d %a\n", fits ? 1 : 0, fits && fit_i ? 1 : 0, fits ? score : 0.0);
+      if (!adv) {
+        const bool fits = node_key(d, R, row.data(), row.data() + R, 1, a_gpu, a_cpu, gpu_count, nflags, n, score, fit_i);
+        printf("K %d %d %a\n", fits ? 1 : 0, fits && fit_i ? 1 : 0, fits ? score : 0.0);
+        continue;
+      }
+      const size_t a = 14 + 3 * (size_t)R;
+      d.pipeline_only = (int)I(a);
+      Tile tl;
+      memset(&tl, 0, sizeof(tl));
+      int node = n, rank = 0;
+      tl.I = row.data();
+      tl.L = row.data() + R;
+      tl.Agpu = &a_gpu;
+      tl.Acpu = &a_cpu;
+      tl.gpu_count = &gpu_count;
+      tl.rank = &rank;
+      tl.flags = &nflags;
+      tl.node = &node;
+      tl.npc = tl.count = 1;
+      tl.R = R;
+      double Ik[KAI_MAX_RES], Lk[KAI_MAX_RES];
+      bool to_idle = false, fits_k = false;
+      const bool ok = repeat_row(tl, d, 0, (int)I(a + 1), D(a + 2), 0.0, Ik, Lk, to_idle, fits_k);
+      row_fits(d.req, R, Ik, Lk, 1, fit_i);
+      if (fits_k) score = row_score(d, Ik, Lk, 1, a_gpu, a_cpu, gpu_count, nflags, n, fit_i);
+      printf("A %d %d %d %d %a\n", to_idle ? 1 : 0, ok ? 1 : 0, fits_k ? 1 : 0, fits_k && fit_i ? 1 : 0, fits_k ? score : 0.0);
     } else {
       printf("FAIL unknown case kind %s\n", f[0].c_str());
       return 1;
